@@ -35,7 +35,6 @@ from __future__ import annotations
 
 import argparse
 import ctypes
-import hashlib
 import json
 import os
 import subprocess
@@ -51,15 +50,14 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 METRIC = "gaussians_rasterized_per_sec_fwd_bwd"
 UNIT = "Gaussians/s"
-CSRC = os.path.join(ROOT, "gaussian-splatting-cuda_b200", "csrc")
 KERNEL_NAMES = ("projection_ut", "sh_fwd", "isect_count", "isect_depth_sort", "isect_runs", "isect_tile_hist",
                 "isect_colscan", "isect_emit", "isect_repair", "isect_keys", "isect_sort", "isect_offsets", "raster_prep", "raster_fwd", "raster_bwd", "raster_finalize", "sh_bwd",
                 "sh_bwd_views", "fused_front", "fused_back", "ssim_l1_fwd", "ssim_l1_bwd", "adam_step",
                 "fgs_front", "ewa_blend_fwd", "ewa_blend_bwd", "fgs_back")
 WORKLOADS = {
     "A": "10k synthetic Gaussians, 256x256, SH deg 0, 1 camera (BASELINE.json configs[0])",
-    "B": "1M synthetic Gaussians, 1920x1080, SH deg 3, 16x16 tiles, fwd+bwd on 1xB200 (BASELINE.json configs[1])",
-    "D": "6M synthetic Gaussians, 1920x1080, SH deg 3, 16x16 tiles, fwd+bwd on 1xB200 (BASELINE.json configs[3])",
+    "B": "1M synthetic Gaussians, 1920x1080, SH deg 3, 16x16 tiles, fwd+bwd on 1xH100 (BASELINE.json configs[1])",
+    "D": "6M synthetic Gaussians, 1920x1080, SH deg 3, 16x16 tiles, fwd+bwd on 1xH100 (BASELINE.json configs[3])",
 }
 
 
@@ -74,34 +72,7 @@ def load_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def source_hash(files):
-    h = hashlib.sha256()
-    for f in files:
-        with open(os.path.join(CSRC, f), "rb") as fh:
-            h.update(fh.read())
-    return h.hexdigest()[:16]
-
-
-def ncu_traffic(kernel, n_gauss, width, height):
-    """DRAM bytes per launch of `kernel` from the committed ncu digest (profiles/ncu_traffic.json), or None when the
-    digest was taken from different kernel sources (stale) or another workload."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if not os.path.exists(p):
-        return None, "no capture committed"
-    try:
-        ent = json.load(open(p)).get(kernel)
-        if not ent:
-            return None, "no capture for this kernel"
-        if [ent["gaussians"], ent["width"], ent["height"]] != [n_gauss, width, height]:
-            return None, "capture is for another workload"
-        if ent["source_sha"] != source_hash(ent["sources"]):
-            return None, "stale: kernel sources changed since the capture"
-        return int(ent["dram_bytes_read"] + ent["dram_bytes_write"]), ent.get("capture", "")
-    except Exception as e:  # a malformed digest must not break the bench
-        return None, f"unreadable: {e!r}"[:80]
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -258,7 +229,7 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------
 class TimedBackend:
     """Wraps an OpsBackend: CUDA events on the launching stream around every operator call, so that both libraries are
@@ -295,6 +266,30 @@ class TimedBackend:
         return {k: round(float(np.median(v)), 4) for k, v in agg.items()}
 
 
+DUMP_GAUSSIAN_SAMPLE = 65536
+
+
+def dump_outputs(out_dir, wl, names):
+    """Writes what the last timed step handed its caller as <out_dir>/<name>.npy (float32; the loss in float64): the
+    rendered image and alpha in full, and the parameter gradients on a fixed, seeded sample of Gaussians (all of them
+    would be ~240 MB at 1 M), so that two builds can be compared output for output on the same inputs."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    loss, out = wl.last
+    arrays = {"loss": np.asarray(float(loss.detach().item()), np.float64),
+              "render_colors": out.render_colors.detach().float().cpu().numpy(),
+              "render_alphas": out.alpha.detach().float().cpu().numpy()}
+    n = wl.N
+    idx = np.arange(n) if n <= DUMP_GAUSSIAN_SAMPLE else \
+        np.sort(np.random.default_rng(0).choice(n, DUMP_GAUSSIAN_SAMPLE, replace=False))
+    arrays["gaussian_sample_index"] = idx.astype(np.float64)
+    sel = torch.from_numpy(idx).to(wl.P["means"].device)
+    for k in names:
+        arrays[f"grad_{k}"] = wl.P[k].grad.detach().index_select(0, sel).float().cpu().numpy()
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+
+
 def percentiles(ms):
     a = np.asarray(ms, np.float64)
     return {"n": int(a.size), "median_ms": float(np.median(a)), "p10_ms": float(np.percentile(a, 10)),
@@ -311,7 +306,7 @@ def run_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a CUDA device: the B200 backend has no CPU fallback")
+        raise RuntimeError("bench.py needs a CUDA device: the CUDA backend has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     pg2 = None
@@ -408,6 +403,7 @@ def run_b200(args):
             elif world > 1:
                 multiview.allreduce_gradients([Pd[k].grad for k in names])
             self.stats["n_isects"], self.stats["vis"] = out.n_isects, out.visibility
+            self.last = (loss, out)
             return loss, out
 
         # -- raw SplatData: what training holds (log-scales, logits, raw quaternions, sh0 / shN) --
@@ -525,6 +521,8 @@ def run_b200(args):
     launches0 = cabi.gsb_launch_count()
     ms_total = timed(wl.step, args.steps)
     launches = int(cabi.gsb_launch_count() - launches0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl, names)
     ms_step = ms_total / args.steps
     value = N * world / (ms_step * 1e-3)
     prof = read_profile(wl.step, max(args.steps, 10))  # per-kernel events in a SEPARATE pass
@@ -542,7 +540,7 @@ def run_b200(args):
             "gaussians": N, "visible": int(wl.stats["vis"].sum().item()), "intersections": wl.stats["n_isects"],
             "image": [W, H], "loss": "L1 vs synthetic target", "parallelism": f"view-dp{world}",
             "l2": "per-step working set (236 B/Gaussian parameters + 64 B records + 12 B/intersection lists + 236 B "
-                  "gradients) exceeds the 126 MB L2; no explicit flush"}
+                  "gradients) exceeds the 50 MB L2; no explicit flush"}
     line["config"] = cfgd
     line["intersections_per_sec"] = wl.stats["n_isects"] * world / (ms_step * 1e-3)
 
@@ -553,13 +551,11 @@ def run_b200(args):
     algo = {"raster_bwd": 60 * I + 24 * Pn + 112 * N, "raster_fwd": 48 * I + 20 * Pn}
     if dom in algo:
         achieved = algo[dom] / (prof[dom]["avg_ms"] * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic(dom, N, W, H)
         line["roofline"] = {
             "kernel": dom, "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-            "algorithmic_bytes_per_launch": algo[dom], "avg_kernel_ms": prof[dom]["avg_ms"],
+            "peak_source": peak_src, "algorithmic_bytes_per_launch": algo[dom], "avg_kernel_ms": prof[dom]["avg_ms"],
             "note": "the blend is FP32-issue/LSU/atomic bound by construction (SURVEY.md 8d): the HBM fraction is the "
-                    "figure north_star asks for, the pipe utilisations are in profiles/"}
+                    "figure north_star asks for"}
 
     if args.quick:
         if rank == 0:
@@ -617,7 +613,7 @@ def run_b200(args):
                             "phases_ms": (phases if ms_local is not None else None),
                             "allreduce_236B_ms": ms_ar, "allreduce_bytes": nbytes,
                             "allreduce_bus_GBps": 2.0 * (world - 1) / world * nbytes / (ms_ar * 1e-3) / 1e9,
-                            "nvlink5_peak_GBps_per_direction": 900.0,
+                            "nvlink4_peak_GBps_per_direction": 450.0,
                             "note": "e2e re-uploads the REPLICATED parameters from every rank through one host: "
                                     "e2e_resident (camera + target in, loss out) is the multi-GPU end-to-end figure"}
     if rank != 0 or world > 1:
@@ -677,7 +673,7 @@ def run_b200(args):
                 ms_ref_raw_res = wl.e2e_resident(args.steps, ref_raw)
                 fused_res = line["fused"].get("e2e_resident_ms")
                 line["reference_cuda"] = {
-                    "what": "reference gsplat/*.cu compiled unmodified (-O3 --use_fast_math, sm_100) by oracle/build_ref.py, "
+                    "what": "reference gsplat/*.cu compiled unmodified (-O3 --use_fast_math, sm_90) by oracle/build_ref.py, "
                             "driven through the same L3 call sequence on the same inputs",
                     "ms_per_step": ms_ref, "value": N / (ms_ref * 1e-3), "unit": UNIT, "distribution": dist_ref,
                     "e2e_ms": ms_ref_e2e, "e2e_resident_ms": ms_ref_res,
@@ -826,7 +822,7 @@ def run_b200(args):
                                              "instances": int(c["ints"][1]), "buckets": int(c["ints"][2]),
                                              "distribution": distribution(ref, warm=3, n=30),
                                              "what": "reference fastgs/rasterization/*.cu compiled unmodified (-O3 "
-                                                     "--use_fast_math, sm_100) by oracle/build_ref.py, same call sites"}
+                                                     "--use_fast_math, sm_90) by oracle/build_ref.py, same call sites"}
                     out["speedup"] = ms_r / ms
                     del c
             except Exception as e:
@@ -1026,6 +1022,9 @@ def main():
     ap.add_argument("--no-ref-cuda", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the config A / D block of the N=1 line")
     ap.add_argument("--quick", action="store_true", help="device-resident timing only (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the image, alpha, loss and a seeded sample of the parameter "
+                         "gradients of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.quick:
         args.no_cpu_baseline = args.no_ref_cuda = args.no_other_configs = True

@@ -1,4 +1,4 @@
-"""gaussian-splatting-cuda_b200: B200-native (sm_100a) 3DGUT rasterizer hot path.
+"""gaussian-splatting-cuda_b200: H100-native (sm_90a) 3DGUT rasterizer hot path.
 
 Python host-side mirror used by the tests and bench.py.  The product is the C-ABI CUDA library
 (lib/libgsb200.so, include/gsb200.h) and the libtorch shim exporting the reference's
@@ -52,7 +52,7 @@ def load() -> None:
         if not os.path.exists(p):
             raise NativeLibraryError(
                 f"{p} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(there is no CPU fallback for the B200 backend)")
+                "(there is no CPU fallback for the CUDA backend)")
     torch.ops.load_library(SHIM_PATH)
     _loaded = True
 

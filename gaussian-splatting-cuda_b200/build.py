@@ -1,6 +1,6 @@
-"""In-tree build of the B200 backend (no GPU needed: nvcc cross-compiles sm_100a).
+"""In-tree build of the CUDA backend (no GPU needed: nvcc cross-compiles sm_90a).
 
-Artifacts (all under gaussian-splatting-cuda_b200/lib/, git-ignored, shipped to the GPU box):
+Artifacts (all under gaussian-splatting-cuda_b200/lib/, git-ignored):
   libgsb200.so           the C-ABI CUDA library (include/gsb200.h); no torch dependency
   libgsplat_b200.so      the libtorch shim exporting the reference's gsplat:: operator API
                          (include/gsplat/Ops.h), its fast_gs::rasterization API (include/fastgs/rasterization_api.h)
@@ -13,6 +13,7 @@ import os
 import shutil
 import subprocess
 import sys
+from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -25,7 +26,7 @@ INC = os.path.join(ROOT, "include")
 NVCC = os.environ.get("GSB_NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else (shutil.which("g++") or "g++")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
               "-ccbin", CXX]
 
@@ -81,19 +82,26 @@ def build_cuda(verbose: bool = False, force: bool = False, ptxas_info: bool = Fa
     os.makedirs(LIB, exist_ok=True)
     os.makedirs(OBJ, exist_ok=True)
     hdrs = [os.path.join(CSRC, h) for h in CUDA_HEADERS] + [os.path.join(INC, "gsb200.h")]
-    objs = []
-    logs = []
-    for src, extra in CUDA_SOURCES:
+
+    def compile_one(src_extra) -> tuple[str, str]:
+        src, extra = src_extra
         sp = os.path.join(CSRC, src)
         op = os.path.join(OBJ, src.replace(".cu", ".o"))
         st = _stamp([sp] + hdrs, " ".join(NVCC_FLAGS + ARCH + extra))
+        log = ""
         if force or _needs(op, st) or ptxas_info:
             cmd = [NVCC, "-c", sp, "-o", op] + NVCC_FLAGS + ARCH + extra + ["-I", INC]
             if ptxas_info:
                 cmd += ["-Xptxas", "-v"]
-            logs.append(_run(cmd, verbose))
+            log = _run(cmd, verbose)
             _mark(op, st)
-        objs.append(op)
+        return op, log
+
+    # the translation units are independent: compile them side by side
+    with ThreadPoolExecutor(max_workers=min(len(CUDA_SOURCES), os.cpu_count() or 1)) as ex:
+        done = list(ex.map(compile_one, CUDA_SOURCES))
+    objs = [op for op, _ in done]
+    logs = [log for _, log in done if log]
     out = os.path.join(LIB, "libgsb200.so")
     st = _stamp(objs)
     if force or _needs(out, st):
@@ -120,15 +128,18 @@ def build_shim(verbose: bool = False, force: bool = False) -> str:
         incs += ["-I", i]
     hdrs = [os.path.join(INC, "gsb200.h")] + [os.path.join(INC, "gsplat", h) for h in ("Ops.h", "FusedOps.h", "Common.h", "Cameras.h")] + \
         [os.path.join(INC, "fastgs", "rasterization_api.h"), os.path.join(INC, "fastgs", "rasterization_ext.h")]
-    objs = []
-    for src in SHIM_SOURCES:
+    def compile_one(src: str) -> str:
         sp = os.path.join(SHIM, src)
         op = os.path.join(OBJ, "shim_" + src.replace(".cpp", ".o"))
         st = _stamp([sp] + hdrs, " ".join(flags) + torch.__version__)
         if force or _needs(op, st):
             _run([CXX, "-c", sp, "-o", op] + flags + incs, verbose)
             _mark(op, st)
-        objs.append(op)
+        return op
+
+    # each translation unit parses the torch headers (~20 s): compile them side by side
+    with ThreadPoolExecutor(max_workers=min(len(SHIM_SOURCES), os.cpu_count() or 1)) as ex:
+        objs = list(ex.map(compile_one, SHIM_SOURCES))
     out = os.path.join(LIB, "libgsplat_b200.so")
     st = _stamp(objs + [os.path.join(LIB, "libgsb200.so")])
     if force or _needs(out, st):

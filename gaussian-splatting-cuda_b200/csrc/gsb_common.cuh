@@ -1,6 +1,6 @@
-// gsb_common.cuh -- shared device helpers for the sm_100a 3DGUT hot path.
+// gsb_common.cuh -- shared device helpers for the sm_90a 3DGUT hot path.
 // No torch, no GLM: plain CUDA C++ with a few inline-PTX wrappers
-// (mbarrier, cp.async.bulk, vector red) for the Blackwell async-copy path.
+// (mbarrier, cp.async.bulk, vector red) for the Hopper async-copy (TMA) path.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -146,7 +146,7 @@ __host__ __device__ inline CamPose cam_pose_from_viewmat(const float *v) {
 }
 
 // ------------------------------------------------------------------------------------------
-// PTX wrappers (sm_90+/sm_100a): mbarrier + bulk async copy (TMA unit, non-tensor form).
+// PTX wrappers (sm_90a): mbarrier + bulk async copy (TMA unit, non-tensor form).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -210,42 +210,19 @@ __device__ __forceinline__ float fast_ex2(float x) {
     return r;
 }
 
-// ---- packed fp32 pairs (Blackwell FFMA2 / FMUL2 / FADD2: two IEEE-rn fp32 results per issue slot) ----
-// A scalar operand built with f2_bc() is folded by ptxas into the instruction's broadcast modifier,
-// so mixing per-Gaussian scalars with per-pixel pairs costs no extra moves.
+// ---- fp32 pairs: two pixels' values carried side by side through the blend ----
+// Hopper has no packed fp32 instruction, so each pair operation is two scalar IEEE-rn FFMA / FMUL / FADD
+// (the explicit __f*_rn intrinsics keep ptxas from contracting or reassociating them).  Each lane's
+// result is the same as a packed fp32x2 instruction would give.
 struct f2 {
-    unsigned long long v;
+    float lo, hi;
 };
-__device__ __forceinline__ f2 f2_make(float lo, float hi) {
-    f2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ f2 f2_bc(float a) { return f2_make(a, a); }
-__device__ __forceinline__ float f2_lo(f2 a) {
-    float lo;
-    asm("{ .reg .b32 t; mov.b64 {%0, t}, %1; }" : "=f"(lo) : "l"(a.v));
-    return lo;
-}
-__device__ __forceinline__ float f2_hi(f2 a) {
-    float hi;
-    asm("{ .reg .b32 t; mov.b64 {t, %0}, %1; }" : "=f"(hi) : "l"(a.v));
-    return hi;
-}
-__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) {
-    f2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-    return r;
-}
-__device__ __forceinline__ f2 f2_mul(f2 a, f2 b) {
-    f2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
-__device__ __forceinline__ f2 f2_add(f2 a, f2 b) {
-    f2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
+__device__ __forceinline__ f2 f2_make(float lo, float hi) { return f2{lo, hi}; }
+__device__ __forceinline__ f2 f2_bc(float a) { return f2{a, a}; }
+__device__ __forceinline__ float f2_lo(f2 a) { return a.lo; }
+__device__ __forceinline__ float f2_hi(f2 a) { return a.hi; }
+__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { return f2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ f2 f2_mul(f2 a, f2 b) { return f2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2 f2_add(f2 a, f2 b) { return f2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 
 } // namespace gsb

@@ -1,4 +1,4 @@
-// gsb_devsort.cuh -- device-wide sort / scan primitives of the intersect stage, hand-written for sm_100a.
+// gsb_devsort.cuh -- device-wide sort / scan primitives of the intersect stage, hand-written for sm_90a.
 //
 // Replaces the library calls of the reference's intersect_tile (cub::DeviceRadixSort::SortPairs,
 // gsplat/IntersectTile.cu:300-314; at::cumsum, gsplat/Intersect.cpp:71) with this repository's own
@@ -159,9 +159,8 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(
     }
     __syncthreads();
     // (d) ranked scatter: 32 keys per step, equal digits keep lane (= input) order.  The set of lanes with the same
-    //     digit comes from eight ballots (one per digit bit), not from match.any, which costs ~12 cycles per DISTINCT
-    //     value on sm_100 (391 cycles for 32 different digits, profiles/r2_ubench.md); the next step's key is loaded
-    //     before this step's rank is computed.
+    //     digit comes from eight ballots (one per digit bit), not from match.any, whose cost grows with the number of
+    //     DISTINCT values in the warp; the next step's key is loaded before this step's rank is computed.
     uint32_t *cur = s_w[warp];
     KeyT key_next = 0;
     if (wlo + lane < whi) key_next = ksrc[wlo + lane];

@@ -1,5 +1,5 @@
 // gsb_fastgs.cu -- SURVEY.md 8 f4: the reference's default rasterizer ("fastgs": EWA splatting of 2-D conics) on the
-// B200 blend engine of this library.
+// blend engine of this library.
 //
 // Replaces fast_gs::rasterization::forward / backward (reference: fastgs/rasterization/src/forward.cu:15-199,
 // src/backward.cu:14-116, include/kernels_forward.cuh, include/kernels_backward.cuh, include/kernel_utils.cuh) behind the

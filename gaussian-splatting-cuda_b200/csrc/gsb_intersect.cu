@@ -787,9 +787,9 @@ struct DeviceShape {
     int smem_sm;    // shared memory per SM
 };
 static const DeviceShape &device_shape() {
-    // immutable after the first call (C++11 thread-safe initialisation); sm_100a: 148 SMs, 227 KB / 228 KB
+    // immutable after the first call (C++11 thread-safe initialisation); sm_90a (H100 SXM): 132 SMs, 227 KB / 228 KB
     static const DeviceShape s = [] {
-        DeviceShape d{148, 227 * 1024, 228 * 1024};
+        DeviceShape d{132, 227 * 1024, 228 * 1024};
         int dev = 0;
         if (cudaGetDevice(&dev) == cudaSuccess) {
             int v = 0;

@@ -155,7 +155,7 @@ extern "C" const char *gsb_error_string(int code) {
     switch (code) {
     case GSB_OK: return "ok";
     case GSB_E_INVALID: return "invalid argument";
-    case GSB_E_UNSUPPORTED: return "configuration not supported by the B200 backend (see DESIGN.md, out of scope)";
+    case GSB_E_UNSUPPORTED: return "configuration not supported by the CUDA backend (see DESIGN.md, out of scope)";
     case GSB_E_WORKSPACE: return "workspace too small or misaligned";
     default: break;
     }

@@ -4,7 +4,7 @@
 // gsplat/Cameras.cuh:1034-1150, gsplat/Utils.cuh:171-179) for the perfect-pinhole / global-shutter
 // camera, the only configuration the reference's callers reach (rasterizer_autograd.cpp:217-237).
 //
-// B200 notes: the kernel is a pure stream (44 B in, <= 36 B out per Gaussian, ~500 FLOP), so the
+// H100 notes: the kernel is a pure stream (44 B in, <= 36 B out per Gaussian, ~500 FLOP), so the
 // design goal is full-sector HBM traffic: a CTA stages its 256-Gaussian slab of the AoS inputs
 // (means/scales 12 B rows, quats 16 B rows, opacities) into shared memory with TMA bulk copies
 // (cp.async.bulk, one per array) and writes the 12-byte conic rows back through shared memory

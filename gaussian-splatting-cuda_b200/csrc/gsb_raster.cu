@@ -4,9 +4,10 @@
 // gsplat/RasterizeToPixelsFromWorld3DGSFwd.cu:20-279, ...Bwd.cu:17-373, gsplat/Utils.cuh:80-194)
 // for the global-shutter camera models of gsb_camera.cuh.  See gsb_raster.cuh for the math.
 //
-// Kernel structure (B200):
+// Kernel structure (H100):
 //   prep      one thread per Gaussian, float64: 64-byte GaussRec (quadratic-form coefficients,
-//             log2 opacity, colour).  N x 64 B stays L2-resident (64 MB at 1 M Gaussians, 126 MB L2).
+//             log2 opacity, colour).  N x 64 B: 64 MB at 1 M Gaussians, more than the H100's 50 MB L2, so
+//             only part of the records stays L2-resident at that size.
 //   fwd       one CTA (4 warps, 128 threads) per 16x16 tile; each thread owns two pixels of an
 //             8x8 sub-block so a warp covers 64 pixels.  The tile's depth-sorted records are
 //             gathered by 64-byte TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) into a
@@ -240,8 +241,6 @@ __global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TilePara
               if (rl < cnt)
                   cand = block_may_pass<kEwa>(rec4[rl * 4], rec4[rl * 4 + 1], rec4[rl * 4 + 2], pc.bx0, pc.bx1, pc.by0, pc.by1);
               uint32_t cmask = __ballot_sync(0xffffffffu, cand);
-              // (evaluating two surviving records per trip to interleave their FFMA2 -> MUFU chains was measured slower:
-              // 0.436 vs 0.420 ms at config B, profiles/r2_experiments.md)
               while (cmask) {
                 const int32_t t = c0 + __ffs(cmask) - 1;
                 cmask &= cmask - 1;
@@ -404,8 +403,7 @@ __global__ void __launch_bounds__(kTileThreads) raster_bwd_kernel(const TilePara
                                                                    float *__restrict__ moments) {
     // Three stages; a stage is filled through its "full" mbarrier (TMA byte count) and released through its "empty"
     // mbarrier (one arrival per warp): no CTA-wide barrier in the loop, a warp with nothing to do in a batch runs ahead
-    // of its neighbours (measured against the two-stage / __syncthreads ring: 0.785 vs 0.799 ms at config B, 1.035 vs
-    // 1.061 ms at 6 M; 64-register / 8-CTA builds of either were slower: profiles/r2_experiments.md).
+    // of its neighbours instead of waiting at a two-stage / __syncthreads ring.
     constexpr int kRing = 3;
     __shared__ __align__(128) GaussRec s_rec[kRing][kBatch];
     __shared__ __align__(8) uint64_t s_full[kRing];

@@ -214,7 +214,7 @@ enum MomentSlot : int {
     kS_W2 = 8, kS_W2X = 9, kS_W2Y = 10, kS_W2XX = 11, kS_W2XY = 12, kS_W2YY = 13, kS_CG = 14, kS_PAD = 15
 };
 
-// chain-rule arithmetic type of the finalize step (float: validated against the f64 oracle, profiles/r1_parity.md)
+// chain-rule arithmetic type of the finalize step (float: validated against the f64 oracle by the parity tests)
 typedef float FT;
 
 // Chain rule from the 15 moments of one Gaussian to the gradients of its ACTIVATED parameters

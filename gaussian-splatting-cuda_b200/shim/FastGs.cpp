@@ -20,7 +20,7 @@ namespace {
 inline gsb_stream_t cur_stream() { return reinterpret_cast<gsb_stream_t>(at::cuda::getCurrentCUDAStream().stream()); }
 
 inline void fgs_check(int rc, const char *op) {
-    TORCH_CHECK(rc == GSB_OK, "fast_gs::rasterization::", op, " (B200 backend) failed: ", gsb_error_string(rc), " [code ", rc,
+    TORCH_CHECK(rc == GSB_OK, "fast_gs::rasterization::", op, " (CUDA backend) failed: ", gsb_error_string(rc), " [code ", rc,
                 "]");
 }
 

@@ -19,7 +19,7 @@ namespace {
 inline gsb_stream_t cur_stream() { return reinterpret_cast<gsb_stream_t>(at::cuda::getCurrentCUDAStream().stream()); }
 
 inline void gsb_check(int rc, const char *op) {
-    TORCH_CHECK(rc == GSB_OK, "gsplat::", op, " (B200 backend) failed: ", gsb_error_string(rc), " [code ", rc, "]");
+    TORCH_CHECK(rc == GSB_OK, "gsplat::", op, " (CUDA backend) failed: ", gsb_error_string(rc), " [code ", rc, "]");
 }
 
 inline const float *opt_f32(const at::optional<at::Tensor> &t) {

@@ -1,4 +1,4 @@
-// Ops.cpp -- the reference's gsplat:: operator API on top of the B200 C ABI (include/gsb200.h).
+// Ops.cpp -- the reference's gsplat:: operator API on top of the C ABI (include/gsb200.h).
 //
 // Host-side mirror of the reference's launch layer (gsplat/{Projection,Intersect,Rasterization,
 // SphericalHarmonics,QuatToRotmat,Relocation}.cpp): same argument checks, same output shapes /
@@ -22,7 +22,7 @@ namespace {
 inline gsb_stream_t cur_stream() { return reinterpret_cast<gsb_stream_t>(at::cuda::getCurrentCUDAStream().stream()); }
 
 inline void gsb_check(int rc, const char *op) {
-    TORCH_CHECK(rc == GSB_OK, "gsplat::", op, " (B200 backend) failed: ", gsb_error_string(rc), " [code ", rc, "]");
+    TORCH_CHECK(rc == GSB_OK, "gsplat::", op, " (CUDA backend) failed: ", gsb_error_string(rc), " [code ", rc, "]");
 }
 
 inline at::Tensor byte_workspace(size_t bytes, const at::Tensor &like) {
@@ -137,7 +137,7 @@ GSB_EXPORT std::tuple<at::Tensor, at::Tensor, at::Tensor> intersect_tile(
     CHECK_INPUT(radii);
     CHECK_INPUT(depths);
     const bool packed = means2d.dim() == 2;
-    TORCH_CHECK(!packed, "gsplat::intersect_tile (B200 backend): packed mode is not supported "
+    TORCH_CHECK(!packed, "gsplat::intersect_tile (CUDA backend): packed mode is not supported "
                          "(the reference's caller rejects it too, rasterizer.cpp:56)");
     (void)camera_ids;
     (void)gaussian_ids;

@@ -1,5 +1,5 @@
 /*
- * gsb200.h -- C ABI of the B200-native (sm_100a) 3DGUT rasterizer hot path.
+ * gsb200.h -- C ABI of the H100-native (sm_90a) 3DGUT rasterizer hot path.
  *
  * This is the drop-in boundary underneath the reference's C++ operator API
  * (namespace gsplat, /root/reference/gsplat/Ops.h:12-165).  Every entry point
@@ -21,7 +21,7 @@
  *    viewer thread (SURVEY.md section 8b).
  *  - return value: GSB_OK (0), a negative GSB_E_* code, or a positive
  *    cudaError_t from a failed launch.  gsb_error_string() names them.
- *  - there is NO CPU fallback: on a machine without an sm_100 device every
+ *  - there is NO CPU fallback: on a machine without an sm_90 device every
  *    compute entry point returns a CUDA error.
  */
 #ifndef GSB200_H_

@@ -4,7 +4,7 @@
 // include/core/camera.hpp:7 and by gsplat's own sources.  Callers outside gsplat/ only use
 // `gsplat::CameraModelType`; the GLM typedefs and the CUB helper in the reference header are
 // internals of its CUDA kernels.  This replacement keeps the public names and values and pulls
-// GLM in only when it is actually installed, because the B200 backend itself does not use GLM.
+// GLM in only when it is actually installed, because the CUDA backend itself does not use GLM.
 #pragma once
 
 #include <algorithm>

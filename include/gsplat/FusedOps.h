@@ -1,4 +1,4 @@
-// FusedOps.h -- EXTENDED operators of the B200 backend (SURVEY.md 8 f1): the hot path over the RAW SplatData
+// FusedOps.h -- EXTENDED operators of the CUDA backend (SURVEY.md 8 f1): the hot path over the RAW SplatData
 // tensors, with the L3 glue of the reference's caller folded in.  Not part of the reference's gsplat/Ops.h; the
 // eleven operators of Ops.h stay available and unchanged.  What a maintainer replaces with one call each:
 //

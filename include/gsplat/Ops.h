@@ -1,4 +1,4 @@
-// Ops.h -- the reference's operator API (namespace gsplat), served by the B200 backend.
+// Ops.h -- the reference's operator API (namespace gsplat), served by the CUDA backend of this library.
 //
 // Signature-for-signature the eleven free functions of /root/reference/gsplat/Ops.h:12-165, which is
 // everything src/training, src/rendering and the strategies reference (SURVEY.md section 8b).  Each

@@ -2,8 +2,8 @@
 
 Compiles the reference's sources WHERE THEY LIE under /root/reference/gsplat (nothing is copied into
 this repo), with the reference's own flags (-O3 --use_fast_math --expt-relaxed-constexpr,
-gsplat/CMakeLists.txt:76) for plain sm_100, plus oracle/ref_binding.cpp, into
-oracle/_ref/libgsplat_ref.so (git-ignored, shipped to the GPU box by gpurun).
+gsplat/CMakeLists.txt:76) for plain sm_90, plus oracle/ref_binding.cpp, into
+oracle/_ref/libgsplat_ref.so (git-ignored).
 
 The reference's device math depends on GLM, which is not vendored in the reference tree and not
 installed here; oracle/glm_shim/ provides the subset it uses (see glm_shim/glm/glm.hpp).
@@ -34,6 +34,12 @@ CPP = ["Projection.cpp", "Intersect.cpp", "SphericalHarmonics.cpp", "QuatToRotma
 TRAIN_CU = ["/root/reference/src/training/kernels/ssim.cu"]
 TRAIN_INC = ["/root/reference/fastgs/optimizer/include"]
 EXTRA = ["ref_binding.cpp", "ref_train_binding.cu"]
+
+
+# Host-only translation units (.cpp) go to the host compiler, as in the reference's own CMake build: through nvcc's
+# device front end the torch headers cost minutes per file, through g++ seconds.
+HOST_FLAGS = ["-O3", "-std=c++20", "-fPIC", "-D_GLIBCXX_USE_CXX11_ABI=1"]
+CUDA_INC = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(NVCC))), "include")
 
 
 def available() -> bool:
@@ -78,13 +84,16 @@ def build(verbose: bool = True, jobs: int = 7, variant: str = "fast") -> str | N
     for i in [os.path.join(HERE, "glm_shim"), REF] + TRAIN_INC + ce.include_paths():
         inc += ["-I", i]
     common = ["-O3", "-std=c++20", "-Xcompiler", "-fPIC", "-D_GLIBCXX_USE_CXX11_ABI=1", "-ccbin", CXX,
-              "-gencode", "arch=compute_100,code=sm_100", "--expt-relaxed-constexpr", f"-DREF_NS={ns}",
+              "-gencode", "arch=compute_90,code=sm_90", "--expt-relaxed-constexpr", f"-DREF_NS={ns}",
               "-diag-suppress", "20012,20011,20014,177,550"] + (["--use_fast_math"] if fast else [])
 
     def compile_one(src: str):
         sp = src if os.path.isabs(src) else os.path.join(REF, src)
         obj = os.path.join(OUT, variant + "_" + os.path.basename(src).rsplit(".", 1)[0] + ".o")
-        cmd = [NVCC, "-c", sp, "-o", obj, "-x", "cu"] + common + inc
+        if sp.endswith(".cpp"):
+            cmd = [CXX, "-c", sp, "-o", obj] + HOST_FLAGS + [f"-DREF_NS={ns}"] + inc + ["-I", CUDA_INC]
+        else:
+            cmd = [NVCC, "-c", sp, "-o", obj] + common + inc
         if verbose:
             print("[build_ref]", os.path.basename(src), flush=True)
         p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -97,7 +106,7 @@ def build(verbose: bool = True, jobs: int = 7, variant: str = "fast") -> str | N
     with ThreadPoolExecutor(max_workers=jobs) as ex:
         objs = list(ex.map(compile_one, srcs))
     tl = ce.library_paths()[0]
-    cmd = [NVCC, "-shared", "-o", so] + objs + ["-gencode", "arch=compute_100,code=sm_100", "-ccbin", CXX, "-L", tl,
+    cmd = [NVCC, "-shared", "-o", so] + objs + ["-gencode", "arch=compute_90,code=sm_90", "-ccbin", CXX, "-L", tl,
                                                  "-ltorch", "-ltorch_cpu", "-lc10", "-ltorch_cuda", "-lc10_cuda",
                                                  "-Xlinker", "-rpath," + tl, "-Xlinker", "-Bsymbolic"]
     p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -220,20 +229,11 @@ FASTGS = "/root/reference/fastgs"
 FASTGS_CU = ["rasterization/src/forward.cu", "rasterization/src/backward.cu", "rasterization/src/rasterization_api.cu"]
 
 
-def build_fastgs(verbose: bool = True, gencode: str = "arch=compute_90,code=compute_90", so_name: str = "libfastgs_ref.so") -> str | None:
+def build_fastgs(verbose: bool = True, gencode: str = "arch=compute_90,code=sm_90", so_name: str = "libfastgs_ref.so") -> str | None:
     """The reference's fastgs rasterizer (SURVEY.md 8 f4), compiled unmodified from where it lies with its own flags
     (fastgs/CMakeLists.txt:58: -O3 --use_fast_math --expt-relaxed-constexpr), plus the product's
     shim/fastgs_binding.cpp compiled against the REFERENCE's rasterization_api.h: oracle/_ref/libfastgs_ref.so,
-    torch.ops.fastgs_ref.*  (the pin of oracle/fastgs_oracle.c and of the B200 path; the same-box GPU baseline).
-
-    Target: compute_90 PTX, JIT-compiled for the B200 by the driver at load time -- NOT sm_100 SASS.  Built for sm_100
-    with this image's CUDA 12.9 CUB, the reference's tile sort (cub::DeviceRadixSort::SortPairs on 16-bit keys,
-    forward.cu:139-145) fails for more than a few hundred thousand instances: a cudaMemsetAsync inside CUB returns
-    "invalid argument", the keys stay unsorted, the bucket count is garbage and forward() asks for terabytes
-    (measured on the B200: 640x368 / 257 k instances fine, 1280x720 / 487 k instances not; compute-sanitizer log in
-    profiles/r2_experiments.md).  The same unmodified sources as compute_90 PTX make CUB select its sm_90 tuning and
-    run correctly at every size tested (1 M and 6 M Gaussians at 1080p); the reference's own kernels use no sm_100
-    feature, so nothing is lost on their side."""
+    torch.ops.fastgs_ref.*  (the pin of oracle/fastgs_oracle.c and of the H100 path; the same-box GPU baseline)."""
     if not os.path.isdir(FASTGS):
         return None
     from torch.utils import cpp_extension as ce
@@ -261,8 +261,11 @@ def build_fastgs(verbose: bool = True, gencode: str = "arch=compute_90,code=comp
         obj = os.path.join(OUT, "fgs_" + so_name + "_" + os.path.basename(src).rsplit(".", 1)[0] + ".o")
         if verbose:
             print("[build_ref] fastgs", os.path.basename(src), flush=True)
-        p = subprocess.run([NVCC, "-c", src, "-o", obj, "-x", "cu"] + common + inc, stdout=subprocess.PIPE,
-                           stderr=subprocess.STDOUT, text=True)
+        if src.endswith(".cpp"):
+            cmd = [CXX, "-c", src, "-o", obj] + HOST_FLAGS + ["-DFGS_REFERENCE_LIBRARY"] + inc + ["-I", CUDA_INC]
+        else:
+            cmd = [NVCC, "-c", src, "-o", obj] + common + inc
+        p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if p.returncode != 0:
             sys.stderr.write(p.stdout[-6000:])
             raise RuntimeError(f"reference fastgs source failed to compile: {src}")
@@ -284,9 +287,16 @@ def build_fastgs(verbose: bool = True, gencode: str = "arch=compute_90,code=comp
     return so
 
 
+def build_all(verbose: bool = True) -> None:
+    """Every reference library.  The three kernel libraries are independent and each takes minutes of nvcc, so they
+    compile side by side; the two caller harnesses link against this repository's shim and come after them."""
+    with ThreadPoolExecutor(max_workers=3) as ex:
+        for f in [ex.submit(build, verbose), ex.submit(build, verbose, variant="precise"), ex.submit(build_fastgs, verbose)]:
+            f.result()
+    with ThreadPoolExecutor(max_workers=2) as ex:
+        for f in [ex.submit(build_l3_harness, verbose), ex.submit(build_fastgs_l3_harness, verbose)]:
+            f.result()
+
+
 if __name__ == "__main__":
-    print(build())
-    print(build(variant="precise"))
-    print(build_l3_harness())
-    print(build_fastgs())
-    print(build_fastgs_l3_harness())
+    build_all()

@@ -20,11 +20,11 @@
  * arithmetic per (pixel, primitive) pair.
  *
  * Pinning: the reference has no test for this path; the pin is the reference's own kernels, compiled unmodified from
- * where they lie (oracle/build_ref.py -> oracle/_ref/libfastgs_ref.so): their outputs on a seeded scene, dumped on a B200
+ * where they lie (oracle/build_ref.py -> oracle/_ref/libfastgs_ref.so): their outputs on a seeded scene, dumped on the GPU
  * by tests/test_gpu_fastgs.py::test_dump_reference_fastgs_golden, are committed as tests/golden/ref_fastgs_small.npz and
  * checked in the no-GPU suite (tests/test_oracle_fastgs.py::test_oracle_vs_reference_fastgs_golden: image 1e-4, every
  * gradient 1e-3, w2c gradient, densification statistics); on the GPU box tests/test_gpu_fastgs.py compares reference
- * kernels, this oracle and the B200 kernels on the same inputs.
+ * kernels, this oracle and this library's kernels on the same inputs.
  *
  * Precision: -DORC_DOUBLE builds the same algorithm in float64.  Gradients are accumulated in float64 either way.
  * -DORC_SMOOTH (test only) drops the three cut-offs (tile bounds / tile test, alpha < 1/255, transmittance < 1e-4) so

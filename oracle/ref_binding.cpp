@@ -1,6 +1,6 @@
 // ref_binding.cpp -- exposes the REFERENCE's own gsplat:: operators (compiled from
 // /root/reference/gsplat by oracle/build_ref.py) as torch.ops.gsplat_ref.* .
-// TEST INFRASTRUCTURE ONLY: the checker that pins the oracle / the B200 path on the rows the
+// TEST INFRASTRUCTURE ONLY: the checker that pins the oracle / the H100 path on the rows the
 // reference's tests do not cover (UT projection, from-world blend fwd/bwd), and the same-box GPU
 // baseline of bench.py.  Same flattening of enums / UT params as the product's torch_binding.cpp.
 #include <torch/library.h>

@@ -1,6 +1,6 @@
 """Backend over the REFERENCE's own fastgs rasterizer (oracle/_ref/libfastgs_ref.so, built by oracle/build_ref.py from
 /root/reference/fastgs/rasterization, unmodified).  TEST INFRASTRUCTURE ONLY: the pin of oracle/fastgs_oracle.c and of
-the B200 fastgs path, and the same-box GPU baseline of bench.py -- driven through the very same Python call sites as the
+the H100 fastgs path, and the same-box GPU baseline of bench.py -- driven through the very same Python call sites as the
 product backend (FastGsBackend of the package)."""
 from __future__ import annotations
 

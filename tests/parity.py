@@ -8,8 +8,7 @@ wrong Gaussians pass, so every gradient comparison additionally bounds, PER GAUS
   * the largest absolute element error relative to the largest reference element.
 The blend is only piecewise continuous (alpha >= 1/255 cut, alpha <= 0.999 gate, T <= 1e-4 stop), so a few
 Gaussians with a pixel at a decision boundary legitimately differ between any two float implementations;
-the bounds are set from the measured float32-vs-float64 noise of the reference formulation itself
-(profiles/r2_parity.md).
+the bounds are set from the measured float32-vs-float64 noise of the reference formulation itself.
 """
 from __future__ import annotations
 

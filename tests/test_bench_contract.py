@@ -1,5 +1,5 @@
 """CPU: the reference arm of bench.py (the oracle port on the host cores) prints ONE JSON line with the
-contract's keys; the B200 arm refuses to run without a CUDA device instead of falling back to the CPU."""
+contract's keys; the GPU arm refuses to run without a CUDA device instead of falling back to the CPU."""
 import json
 import os
 import subprocess

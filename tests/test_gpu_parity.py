@@ -1,4 +1,4 @@
-"""GPU: parity of the sm_100a path (through the gsplat:: shim -> C ABI) against the CPU oracle and
+"""GPU: parity of the sm_90a path (through the gsplat:: shim -> C ABI) against the CPU oracle and
 the committed golden vectors.  Tolerances follow BASELINE.json's north_star: integer / index
 results bit-exact, rendered RGB within 1e-4 relative, gradients within 1e-3 relative.
 

@@ -1,4 +1,4 @@
-"""GPU: the reference's OWN L3 code executes on the B200 through this repository's drop-in library.
+"""GPU: the reference's OWN L3 code executes on the GPU through this repository's drop-in library.
 
 oracle/_ref/libref_l3_b200.so = /root/reference/src/training/rasterization/rasterizer_autograd.cpp compiled unmodified
 (SphericalHarmonicsFunction, fully_fused_projection_with_ut, GUTRasterizationFunction, forward and backward) + a
@@ -22,7 +22,7 @@ SO = os.path.join(ROOT, "oracle", "_ref", "libref_l3_b200.so")
 @pytest.mark.parametrize("name", ["small_rot", "b30k"])
 def test_reference_l3_autograd_runs_on_the_b200_backend(native, cuda_device, name):
     if not os.path.exists(SO):
-        pytest.skip("oracle/_ref/libref_l3_b200.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libref_l3_b200.so not built (build() makes it where the reference's sources are present)")
     torch.ops.load_library(SO)
     sc = {"small_rot": lambda: scenes.scene_small(N=3000, width=200, height=120, view=1),
           "b30k": lambda: scenes.scene_b(N=30000, width=640, height=360, view=3, scale_mul=2.0)}[name]()

@@ -109,7 +109,7 @@ def test_densification_info_accumulates():
 
 def test_oracle_vs_reference_fastgs_golden():
     """Pins the oracle to the REFERENCE'S OWN fastgs kernels without a GPU: tests/golden/ref_fastgs_small.npz was produced on
-    a B200 by tests/test_gpu_fastgs.py::test_dump_reference_fastgs_golden from oracle/_ref/libfastgs_ref.so, i.e.
+    the GPU by tests/test_gpu_fastgs.py::test_dump_reference_fastgs_golden from oracle/_ref/libfastgs_ref.so, i.e.
     /root/reference/fastgs/rasterization/src/*.cu compiled unmodified (oracle/build_ref.py).  Scene:
     scenes.scene_small(N=1500, 176x112, SH degree 3, seed 13, view 2) -> scenes.fastgs_inputs; cotangents from numpy
     default_rng(17)."""

@@ -1,7 +1,7 @@
 """CPU: pin the oracle on the rows the reference's tests do not cover (UT projection, from-world
 blend forward / backward) against outputs of the REFERENCE'S OWN CUDA KERNELS.
 
-tests/golden/ref_cuda_small.npz was produced on a B200 by tests/test_gpu_vs_reference.py::
+tests/golden/ref_cuda_small.npz was produced on the GPU by tests/test_gpu_vs_reference.py::
 test_dump_reference_golden from oracle/_ref/libgsplat_ref.so, i.e. /root/reference/gsplat/*.cu compiled
 unmodified with the reference's flags (oracle/build_ref.py).  Scene: scenes.scene_small(N=1200, 160x96,
 SH deg 3, view=2), colours / cotangents from numpy default_rng(11)."""
