@@ -210,10 +210,9 @@ __device__ __forceinline__ float fast_ex2(float x) {
     return r;
 }
 
-// ---- fp32 pairs: two pixels' values carried side by side through the blend ----
-// Hopper has no packed fp32 instruction, so each pair operation is two scalar IEEE-rn FFMA / FMUL / FADD
-// (the explicit __f*_rn intrinsics keep ptxas from contracting or reassociating them).  Each lane's
-// result is the same as a packed fp32x2 instruction would give.
+// ---- fp32 pairs: two values carried side by side (the SSIM window sums of gsb_loss.cu) ----
+// Each pair operation is two scalar IEEE-rn FFMA / FMUL / FADD (the explicit __f*_rn intrinsics keep
+// ptxas from contracting or reassociating them).
 struct f2 {
     float lo, hi;
 };

@@ -8,18 +8,25 @@
 //   prep      one thread per Gaussian, float64: 64-byte GaussRec (quadratic-form coefficients,
 //             log2 opacity, colour).  N x 64 B: 64 MB at 1 M Gaussians, more than the H100's 50 MB L2, so
 //             only part of the records stays L2-resident at that size.
-//   fwd       one CTA (4 warps, 128 threads) per 16x16 tile; each thread owns two pixels of an
-//             8x8 sub-block so a warp covers 64 pixels.  The tile's depth-sorted records are
-//             gathered by 64-byte TMA bulk copies (cp.async.bulk -> mbarrier complete_tx) into a
-//             two-stage shared-memory ring; ids are prefetched one batch ahead so the gather of
-//             batch b+1 overlaps the blending of batch b.  Per pair: MUFU-free rejection test,
-//             then warp-vote: only warps with a surviving lane pay for rcp/ex2 and the colour row.
-//             A warp whose 64 pixels are saturated stops blending; the CTA leaves when all are.
-//   bwd       same tiling, back-to-front from the CTA-wide max(last_ids), three-stage ring released by per-warp
-//             mbarrier arrivals (no CTA barrier per batch); 15 moments per pair are
-//             summed over the thread's two pixels, reduced across the warp with a 16-value
-//             butterfly (16 shuffles instead of 15 x 5) and added to a per-Gaussian 64-byte row
-//             with one 16-lane red.global.add.f32.
+//   fwd       one CTA (4 warps, 128 threads) per 16x16 tile; each thread owns two pixels of one
+//             column (rows r and r+4) of an 8x8 sub-block, so a warp covers 64 pixels.  The tile's
+//             depth-sorted records are gathered by 64-byte TMA bulk copies (cp.async.bulk -> mbarrier
+//             complete_tx) into a two-stage shared-memory ring; ids are prefetched one batch ahead so
+//             the gather of batch b+1 overlaps the blending of batch b.  Per (record, thread): the
+//             column terms of the rejection test once, then two FFMAs per polynomial per pixel
+//             (gsb_raster.cuh, eval_pixels); a warp-vote lets only warps with a surviving pixel pay
+//             for rcp/ex2 and the colour row.  A warp whose pixels are saturated stops blending; the
+//             CTA leaves when all are.
+//   bwd       one CTA (2 warps, 64 threads) per tile; each thread owns four pixels of one column
+//             (rows r, r+4, r+8, r+12), so a warp covers an 8x16 half tile and the per-event costs
+//             (vote, record loads, warp reduction, reds) are paid once per 128 pixels.  Back-to-front
+//             from the CTA-wide max(last_ids), three-stage ring released by per-warp mbarrier arrivals
+//             (no CTA barrier per batch).  The 15 moments of an event are built on the shared column
+//             from per-thread sums  S0 = sum w, S1 = sum w y, S2 = sum w y^2  (slots S0, x S0, S1,
+//             x^2 S0, x S1, S2), reduced across the warp with a 16-value butterfly (16 shuffles
+//             instead of 15 x 5) and added to a per-Gaussian 64-byte row with one 16-lane
+//             red.global.add.f32.  An image too small to fill the GPU with such CTAs runs the same
+//             kernel with two pixels per thread (4 warps, 128 threads per tile).
 //   finalize  one thread per Gaussian, float32 chain rule from the moments to
 //             (v_means, v_quats, v_scales, v_opacities, v_colors); writes every output element.
 #include "gsb_raster.cuh"
@@ -27,9 +34,12 @@
 namespace gsb {
 
 constexpr int kPrepThreads = 128;
-constexpr int kTileThreads = 128; // 4 warps x 64 pixels
-constexpr int kBatch = 128;       // records per pipeline stage (one per thread)
-constexpr int kStages = 2;
+// pixels per thread and threads per CTA of the blend kernels; a stage of the record ring holds one record per thread
+constexpr int kFwdPix = 2;
+constexpr int kFwdThreads = 256 / kFwdPix;
+// The backward runs four pixels per thread (64 threads per tile) where the image has enough tiles to fill the GPU,
+// else two (128 threads per tile): see launch_bwd.
+constexpr int kBwdPix = 4, kBwdPixSmall = 2;
 
 // ------------------------------------------------------------------------------------------
 // prep
@@ -85,54 +95,65 @@ struct TileParams {
     int32_t n_radial, n_tangential, n_thin_prism;
 };
 
+// A thread owns kPix pixels of one tile column, rows r, r+4, ..., r+4(kPix-1): a warp covers an 8-wide,
+// 4*kPix-tall block and a 16x16 tile takes 256/kPix threads (warp w: column half w & 1, row block w >> 1).
+template <int kPix>
 struct PixelMap {
-    uint32_t x, y0, y1; // pixel coordinates (two rows, same column)
-    bool in0, in1;
+    uint32_t x, y[kPix];
+    bool in[kPix];
 };
-__device__ __forceinline__ PixelMap pixel_map(uint32_t tile_x, uint32_t tile_y, uint32_t W, uint32_t H) {
+template <int kPix>
+__device__ __forceinline__ PixelMap<kPix> pixel_map(uint32_t tile_x, uint32_t tile_y, uint32_t W, uint32_t H) {
     const uint32_t w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    PixelMap m;
+    PixelMap<kPix> m;
     m.x = tile_x * 16 + (w & 1) * 8 + (l & 7);
-    m.y0 = tile_y * 16 + (w >> 1) * 8 + (l >> 3);
-    m.y1 = m.y0 + 4;
-    m.in0 = (m.x < W) && (m.y0 < H);
-    m.in1 = (m.x < W) && (m.y1 < H);
+    const uint32_t y0 = tile_y * 16 + (w >> 1) * (4 * kPix) + (l >> 3);
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        m.y[i] = y0 + 4 * i;
+        m.in[i] = (m.x < W) && (m.y[i] < H);
+    }
     return m;
 }
 
 // Per-thread pixel coordinates in the units of GaussRec (x = px - pcx).  Perfect pinhole: the pixel
-// centres themselves.  General camera: the pixel's ray is unprojected through the camera model
-// (Newton undistortion / fisheye polynomial inverse) once per pixel and mapped back through the ideal
-// pinhole, px = fx * x_n + cx; the warp's cull box is the bounding box of its valid pixels.
+// centres themselves, so px[] holds one value.  General camera: the pixel's ray is unprojected through
+// the camera model (Newton undistortion / fisheye polynomial inverse) once per pixel and mapped back
+// through the ideal pinhole, px = fx * x_n + cx; the warp's cull box is the bounding box of its valid pixels.
+template <int kPix>
 struct PixelCoords {
-    float px0, py0, px1, py1;
-    bool ok0, ok1;            // ray valid (Fwd.cu:139, Bwd.cu:151)
+    float px[kPix], py[kPix];
+    bool ok[kPix];            // ray valid (Fwd.cu:139, Bwd.cu:151)
     float bx0, bx1, by0, by1; // cull box of the warp
 };
-template <bool kGeneral>
-__device__ __forceinline__ PixelCoords pixel_coords(const TileParams &p, const PixelMap &pm, uint32_t tile_x,
-                                                    uint32_t tile_y, const CamModel *cm) {
-    PixelCoords c;
-    const uint32_t tid = threadIdx.x;
-    c.px0 = c.px1 = (float)pm.x + 0.5f;
-    c.py0 = (float)pm.y0 + 0.5f;
-    c.py1 = (float)pm.y1 + 0.5f;
-    c.ok0 = c.ok1 = true;
-    c.bx0 = (float)(tile_x * 16 + ((tid >> 5) & 1) * 8) + 0.5f;
-    c.by0 = (float)(tile_y * 16 + (tid >> 6) * 8) + 0.5f;
+template <bool kGeneral, int kPix>
+__device__ __forceinline__ PixelCoords<kPix> pixel_coords(const PixelMap<kPix> &pm, uint32_t tile_x, uint32_t tile_y,
+                                                          const CamModel *cm) {
+    PixelCoords<kPix> c;
+    const uint32_t w = threadIdx.x >> 5;
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        c.px[i] = (float)pm.x + 0.5f;
+        c.py[i] = (float)pm.y[i] + 0.5f;
+        c.ok[i] = true;
+    }
+    c.bx0 = (float)(tile_x * 16 + (w & 1) * 8) + 0.5f;
+    c.by0 = (float)(tile_y * 16 + (w >> 1) * (4 * kPix)) + 0.5f;
     c.bx1 = c.bx0 + 7.0f;
-    c.by1 = c.by0 + 7.0f;
+    c.by1 = c.by0 + (float)(4 * kPix - 1);
     if constexpr (kGeneral) {
-        float xn, yn;
-        c.ok0 = cam_unproject_normalized(*cm, c.px0, c.py0, xn, yn);
-        c.px0 = fmaf(cm->fx, xn, cm->cx); c.py0 = fmaf(cm->fy, yn, cm->cy);
-        c.ok1 = cam_unproject_normalized(*cm, c.px1, c.py1, xn, yn);
-        c.px1 = fmaf(cm->fx, xn, cm->cx); c.py1 = fmaf(cm->fy, yn, cm->cy);
         const float BIG = 3.0e38f;
-        float lox = fminf(c.ok0 && pm.in0 ? c.px0 : BIG, c.ok1 && pm.in1 ? c.px1 : BIG);
-        float hix = fmaxf(c.ok0 && pm.in0 ? c.px0 : -BIG, c.ok1 && pm.in1 ? c.px1 : -BIG);
-        float loy = fminf(c.ok0 && pm.in0 ? c.py0 : BIG, c.ok1 && pm.in1 ? c.py1 : BIG);
-        float hiy = fmaxf(c.ok0 && pm.in0 ? c.py0 : -BIG, c.ok1 && pm.in1 ? c.py1 : -BIG);
+        float lox = BIG, hix = -BIG, loy = BIG, hiy = -BIG;
+#pragma unroll
+        for (int i = 0; i < kPix; ++i) {
+            float xn, yn;
+            c.ok[i] = cam_unproject_normalized(*cm, c.px[i], c.py[i], xn, yn);
+            c.px[i] = fmaf(cm->fx, xn, cm->cx); c.py[i] = fmaf(cm->fy, yn, cm->cy);
+            if (c.ok[i] && pm.in[i]) {
+                lox = fminf(lox, c.px[i]); hix = fmaxf(hix, c.px[i]);
+                loy = fminf(loy, c.py[i]); hiy = fmaxf(hiy, c.py[i]);
+            }
+        }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             lox = fminf(lox, __shfl_xor_sync(0xffffffffu, lox, o));
@@ -164,26 +185,29 @@ __device__ __forceinline__ void issue_batch(GaussRec *stage, uint64_t *bar, cons
 // forward
 // ------------------------------------------------------------------------------------------
 template <bool kGeneral, bool kEwa = false>
-__global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TileParams p, float *__restrict__ renders,
-                                                                   float *__restrict__ alphas,
-                                                                   int32_t *__restrict__ last_ids) {
+__global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParams p, float *__restrict__ renders,
+                                                                  float *__restrict__ alphas,
+                                                                  int32_t *__restrict__ last_ids) {
+    constexpr int kPix = kFwdPix, kBatch = kFwdThreads, kStages = 2;
     __shared__ __align__(128) GaussRec s_rec[kStages][kBatch];
     __shared__ __align__(8) uint64_t s_full[kStages];
     __shared__ CamModel s_cm;
 
     const uint32_t tile_id = blockIdx.x;
     const uint32_t tile_y = tile_id / p.tile_w, tile_x = tile_id % p.tile_w;
-    const PixelMap pm = pixel_map(tile_x, tile_y, p.W, p.H);
+    const PixelMap<kPix> pm = pixel_map<kPix>(tile_x, tile_y, p.W, p.H);
     const uint32_t tid = threadIdx.x;
     const bool has_bg = p.backgrounds != nullptr;
     const float bg0 = has_bg ? p.backgrounds[0] : 0.f;
     const float bg1 = has_bg ? p.backgrounds[1] : 0.f;
     const float bg2 = has_bg ? p.backgrounds[2] : 0.f;
 
-    const size_t pix0 = (size_t)pm.y0 * p.W + pm.x, pix1 = (size_t)pm.y1 * p.W + pm.x;
     if (p.masks != nullptr && !p.masks[tile_id]) { // Fwd.cu:143-150: background only, alpha/last_ids untouched
-        if (pm.in0) { renders[pix0 * 3] = bg0; renders[pix0 * 3 + 1] = bg1; renders[pix0 * 3 + 2] = bg2; }
-        if (pm.in1) { renders[pix1 * 3] = bg0; renders[pix1 * 3 + 1] = bg1; renders[pix1 * 3 + 2] = bg2; }
+#pragma unroll
+        for (int i = 0; i < kPix; ++i) {
+            const size_t pix = (size_t)pm.y[i] * p.W + pm.x;
+            if (pm.in[i]) { renders[pix * 3] = bg0; renders[pix * 3 + 1] = bg1; renders[pix * 3 + 2] = bg2; }
+        }
         return;
     }
 
@@ -201,12 +225,23 @@ __global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TilePara
     }
     __syncthreads();
 
-    const PixelCoords pc = pixel_coords<kGeneral>(p, pm, tile_x, tile_y, &s_cm);
-    // blend state of the thread's two pixels as packed pairs (lo = pixel 0, hi = pixel 1)
-    f2 T = f2_bc(1.0f), CR = f2_bc(0.0f), CG = f2_bc(0.0f), CB = f2_bc(0.0f);
-    int32_t last0 = 0, last1 = 0;
-    bool done0 = !pm.in0 || !pc.ok0, done1 = !pm.in1 || !pc.ok1;
-    const f2 PX = f2_make(pc.px0, pc.px1), PY = f2_make(pc.py0, pc.py1);
+    const PixelCoords<kPix> pc = pixel_coords<kGeneral, kPix>(pm, tile_x, tile_y, &s_cm);
+    // blend state of the thread's pixels
+    float T[kPix], CR[kPix], CG[kPix], CB[kPix];
+    int32_t last[kPix];
+    bool done[kPix];
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        T[i] = 1.0f; CR[i] = CG[i] = CB[i] = 0.0f;
+        last[i] = 0;
+        done[i] = !pm.in[i] || !pc.ok[i];
+    }
+    auto all_done = [&]() {
+        bool d = true;
+#pragma unroll
+        for (int i = 0; i < kPix; ++i) d = d && done[i];
+        return d;
+    };
 
     // prologue: batch 0 in flight, ids of batch 1 prefetched into a register
     int32_t gid_next = 0;
@@ -232,10 +267,10 @@ __global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TilePara
 
         const int32_t cnt = min(total - b * kBatch, kBatch);
         const int32_t batch_start = range_start + b * kBatch;
-        if (!__all_sync(0xffffffffu, done0 && done1)) { // this warp's 64 pixels are not all saturated
+        if (!__all_sync(0xffffffffu, all_done())) { // this warp's pixels are not all saturated
             const float4 *rec4 = reinterpret_cast<const float4 *>(s_rec[st]);
             for (int32_t c0 = 0; c0 < cnt; c0 += 32) {
-              // lane-parallel culling of 32 records against this warp's 8x8 pixel block
+              // lane-parallel culling of 32 records against this warp's pixel block
               const int32_t rl = c0 + (int32_t)(tid & 31);
               bool cand = false;
               if (rl < cnt)
@@ -245,54 +280,58 @@ __global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TilePara
                 const int32_t t = c0 + __ffs(cmask) - 1;
                 cmask &= cmask - 1;
                 const float4 q0 = rec4[t * 4], q1 = rec4[t * 4 + 1], q2 = rec4[t * 4 + 2];
-                const PairEval2 e = pair_eval2<kEwa>(q0, q1, q2, f2_add(PX, f2_bc(-q0.x)), f2_add(PY, f2_bc(-q0.y)));
-                const bool p0 = e.pass0 && !done0, p1 = e.pass1 && !done1;
-                if (!__any_sync(0xffffffffu, p0 || p1)) continue;
+                ColTerms c[kGeneral ? kPix : 1];
+                PixEval e[kPix];
+                eval_pixels<kEwa, !kGeneral, kPix>(q0, q1, q2, pc.px, pc.py, c, e);
+                bool pass[kPix], any = false;
+#pragma unroll
+                for (int i = 0; i < kPix; ++i) { pass[i] = e[i].pass && !done[i]; any = any || pass[i]; }
+                if (!__any_sync(0xffffffffu, any)) continue;
                 const float4 q3 = rec4[t * 4 + 3];
-                // Both pixels branch-free on packed pairs (the warp executes both sides of a per-pixel branch anyway:
-                // 40 of 64 pixels pass per event).  A pixel that does not contribute gets alpha = 0: T and colour stay.
-                f2 ex;
-                if constexpr (kEwa) ex = f2_add(e.Ns, f2_bc(q2.z));
-                else ex = f2_fma(e.Ns, f2_make(fast_rcp(f2_lo(e.Ds)), fast_rcp(f2_hi(e.Ds))), f2_bc(q2.z));
-                const float al0 = fminf(kMaxAlpha, fast_ex2(f2_lo(ex))), al1 = fminf(kMaxAlpha, fast_ex2(f2_hi(ex)));
-                const bool ok0 = p0 && al0 >= kAlphaThreshold, ok1 = p1 && al1 >= kAlphaThreshold;
-                f2 alpha = f2_make(ok0 ? al0 : 0.0f, ok1 ? al1 : 0.0f);
-                const f2 nT = f2_mul(T, f2_fma(alpha, f2_bc(-1.0f), f2_bc(1.0f)));
-                // a Gaussian that would push the transmittance to 1e-4 is NOT composited and ends the pixel (Fwd.cu:244-248)
-                const bool sat0 = ok0 && f2_lo(nT) <= kMinTransmittance, sat1 = ok1 && f2_hi(nT) <= kMinTransmittance;
-                alpha = f2_make(sat0 ? 0.0f : f2_lo(alpha), sat1 ? 0.0f : f2_hi(alpha));
-                const f2 vis = f2_mul(alpha, T);
-                CR = f2_fma(f2_bc(q3.x), vis, CR); CG = f2_fma(f2_bc(q3.y), vis, CG); CB = f2_fma(f2_bc(q3.z), vis, CB);
-                T = f2_make(sat0 ? f2_lo(T) : f2_lo(nT), sat1 ? f2_hi(T) : f2_hi(nT));
-                if (ok0 && !sat0) last0 = batch_start + t;
-                if (ok1 && !sat1) last1 = batch_start + t;
-                done0 = done0 || sat0; done1 = done1 || sat1;
+                // Every pixel branch-free (the warp executes both sides of a per-pixel branch anyway: most pixels
+                // pass per event).  A pixel that does not contribute gets alpha = 0: T and colour stay.
+#pragma unroll
+                for (int i = 0; i < kPix; ++i) {
+                    float ex;
+                    if constexpr (kEwa) ex = __fadd_rn(e[i].Ns, q2.z);
+                    else ex = __fmaf_rn(e[i].Ns, fast_rcp(e[i].Ds), q2.z);
+                    const float al = fminf(kMaxAlpha, fast_ex2(ex));
+                    const bool ok = pass[i] && al >= kAlphaThreshold;
+                    float alpha = ok ? al : 0.0f;
+                    const float nT = __fmul_rn(T[i], __fmaf_rn(alpha, -1.0f, 1.0f));
+                    // a Gaussian that would push the transmittance to 1e-4 is NOT composited and ends the pixel
+                    // (Fwd.cu:244-248)
+                    const bool sat = ok && nT <= kMinTransmittance;
+                    if (sat) alpha = 0.0f;
+                    const float vis = __fmul_rn(alpha, T[i]);
+                    CR[i] = __fmaf_rn(q3.x, vis, CR[i]);
+                    CG[i] = __fmaf_rn(q3.y, vis, CG[i]);
+                    CB[i] = __fmaf_rn(q3.z, vis, CB[i]);
+                    if (!sat) T[i] = nT;
+                    if (ok && !sat) last[i] = batch_start + t;
+                    done[i] = done[i] || sat;
+                }
               }
-              if (__all_sync(0xffffffffu, done0 && done1)) break;
+              if (__all_sync(0xffffffffu, all_done())) break;
             }
         }
         // releases stage `st` for batch b+2 and tells every warp whether the tile is saturated
-        if (__syncthreads_and(done0 && done1)) { saturated = true; break; }
+        if (__syncthreads_and(all_done())) { saturated = true; break; }
     }
     // never retire the CTA with a bulk copy still landing in its shared memory
     if (saturated && b + 1 < n_batches) mbar_wait(&s_full[(b + 1) & 1], (uint32_t)(((b + 1) >> 1) & 1));
 
     // [H,W,3] rows (gsplat operators) or [3,H,W] planes (fastgs API)
     const size_t cs = p.chw ? (size_t)p.W * p.H : 1, ps = p.chw ? 1 : 3;
-    const float T0 = f2_lo(T), T1 = f2_hi(T);
-    if (pm.in0) {
-        alphas[pix0] = 1.0f - T0;
-        renders[pix0 * ps] = has_bg ? f2_lo(CR) + T0 * bg0 : f2_lo(CR);
-        renders[pix0 * ps + cs] = has_bg ? f2_lo(CG) + T0 * bg1 : f2_lo(CG);
-        renders[pix0 * ps + 2 * cs] = has_bg ? f2_lo(CB) + T0 * bg2 : f2_lo(CB);
-        last_ids[pix0] = last0;
-    }
-    if (pm.in1) {
-        alphas[pix1] = 1.0f - T1;
-        renders[pix1 * ps] = has_bg ? f2_hi(CR) + T1 * bg0 : f2_hi(CR);
-        renders[pix1 * ps + cs] = has_bg ? f2_hi(CG) + T1 * bg1 : f2_hi(CG);
-        renders[pix1 * ps + 2 * cs] = has_bg ? f2_hi(CB) + T1 * bg2 : f2_hi(CB);
-        last_ids[pix1] = last1;
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        if (!pm.in[i]) continue;
+        const size_t pix = (size_t)pm.y[i] * p.W + pm.x;
+        alphas[pix] = 1.0f - T[i];
+        renders[pix * ps] = has_bg ? CR[i] + T[i] * bg0 : CR[i];
+        renders[pix * ps + cs] = has_bg ? CG[i] + T[i] * bg1 : CG[i];
+        renders[pix * ps + 2 * cs] = has_bg ? CB[i] + T[i] * bg2 : CB[i];
+        last_ids[pix] = last[i];
     }
 }
 
@@ -300,120 +339,155 @@ __global__ void __launch_bounds__(kTileThreads) raster_fwd_kernel(const TilePara
 // backward
 // ------------------------------------------------------------------------------------------
 
-// Per-thread state of the backward sweep for the thread's two pixels (lo = pixel 0, hi = pixel 1).
-struct BwdState {
-    f2 T;      // running transmittance (restored front-to-back value at the current Gaussian)
-    f2 bdot;   // (colour accumulated behind) . dL/d(colour)
-    f2 tfva;   // T_final * (dL/d(alpha) - bg . dL/d(colour))
-    f2 vr, vg, vb; // dL/d(render colour)
-    f2 vA, vB, vC, vD; // the colour slots' per-pixel factors, pre-swapped for lanes 16..31 (see MomentSlot)
-    int32_t last0, last1;
-    bool in0, in1;
+// Per-pixel state of the backward sweep.
+struct BwdPixel {
+    float T;          // running transmittance (restored front-to-back value at the current Gaussian)
+    float bdot;       // (colour accumulated behind) . dL/d(colour)
+    float tfva;       // T_final * (dL/d(alpha) - bg . dL/d(colour))
+    float vr, vg, vb; // dL/d(render colour)
+    int32_t last;
+    bool in;
 };
 
-__device__ __forceinline__ float f2_sum(f2 a) { return f2_lo(a) + f2_hi(a); }
-
-// One (record, pixel pair) event of the backward sweep, branch-free over the two pixels: a pixel that
-// does not contribute gets alpha = 0, which leaves its state untouched and yields zero weights.
+// One (record, pixel) event of the backward sweep, branch-free: a pixel that does not contribute gets
+// alpha = 0, which leaves its state untouched and yields zero weights.
 //   w1 = dL/dNs, w2 = dL/dDs, g = dL/d(power), fac = alpha * T (weight of dL/d(colour))
 struct EventWeights {
-    f2 w1, w2, g, fac;
+    float w1, w2, g, fac;
 };
 template <bool kEwa = false>
-__device__ __forceinline__ EventWeights bwd_weights(BwdState &s, const PairEval2 &e, bool p0, bool p1, float lop,
-                                                    float cr, float cg, float cb) {
-    f2 rD, ex; // same rounding as the forward's pair_alpha_raw
+__device__ __forceinline__ EventWeights bwd_weights(BwdPixel &s, const PixEval &e, bool pass, float lop, float cr,
+                                                    float cg, float cb) {
+    float rD, ex; // same rounding as the forward
     if constexpr (kEwa) {
-        rD = f2_bc(1.0f);
-        ex = f2_add(e.Ns, f2_bc(lop));
+        rD = 1.0f;
+        ex = __fadd_rn(e.Ns, lop);
     } else {
-        rD = f2_make(fast_rcp(f2_lo(e.Ds)), fast_rcp(f2_hi(e.Ds)));
-        ex = f2_fma(e.Ns, rD, f2_bc(lop));
+        rD = fast_rcp(e.Ds);
+        ex = __fmaf_rn(e.Ns, rD, lop);
     }
-    const float ar0 = fast_ex2(f2_lo(ex)), ar1 = fast_ex2(f2_hi(ex));
-    const float al0 = fminf(kMaxAlpha, ar0), al1 = fminf(kMaxAlpha, ar1);
-    const bool ok0 = p0 && al0 >= kAlphaThreshold, ok1 = p1 && al1 >= kAlphaThreshold;
-    const f2 alpha = f2_make(ok0 ? al0 : 0.0f, ok1 ? al1 : 0.0f);
+    const float ar = fast_ex2(ex);
+    const float al = fminf(kMaxAlpha, ar);
+    const bool ok = pass && al >= kAlphaThreshold;
+    const float alpha = ok ? al : 0.0f;
     // Bwd.cu:318: the gradient reaches the Gaussian through alpha only when alpha was not clamped
     // (the fastgs blend differentiates through the clamped value: kernels_backward.cuh:421-426 has no such test)
-    const f2 araw_g = kEwa ? alpha
-                           : f2_make((ok0 && ar0 <= kMaxAlpha) ? ar0 : 0.0f, (ok1 && ar1 <= kMaxAlpha) ? ar1 : 0.0f);
-    const f2 om = f2_fma(alpha, f2_bc(-1.0f), f2_bc(1.0f));
+    const float araw_g = kEwa ? alpha : ((ok && ar <= kMaxAlpha) ? ar : 0.0f);
+    const float om = __fmaf_rn(alpha, -1.0f, 1.0f);
     // the reference evaluates 1/(1-alpha) with the fast-math reciprocal too (Bwd.cu:291 under --use_fast_math)
-    float ra0 = 1.0f, ra1 = 1.0f;
-    if (ok0) ra0 = fast_rcp(f2_lo(om));
-    if (ok1) ra1 = fast_rcp(f2_hi(om));
-    const f2 ra = f2_make(ra0, ra1);
-    s.T = f2_mul(s.T, ra);
+    const float ra = ok ? fast_rcp(om) : 1.0f;
+    s.T = __fmul_rn(s.T, ra);
     EventWeights w;
-    w.fac = f2_mul(alpha, s.T);
+    w.fac = __fmul_rn(alpha, s.T);
     // v_alpha = sum_c (c_c T - behind_c / (1-alpha)) v_c + T_final (...) / (1-alpha)     (Bwd.cu:296-316)
-    const f2 cv = f2_fma(f2_bc(cr), s.vr, f2_fma(f2_bc(cg), s.vg, f2_mul(f2_bc(cb), s.vb)));
-    const f2 v_alpha = f2_fma(s.T, cv, f2_mul(ra, f2_fma(s.bdot, f2_bc(-1.0f), s.tfva)));
-    s.bdot = f2_fma(w.fac, cv, s.bdot);
-    w.g = f2_mul(araw_g, v_alpha);
+    const float cv = __fmaf_rn(cr, s.vr, __fmaf_rn(cg, s.vg, __fmul_rn(cb, s.vb)));
+    const float v_alpha = __fmaf_rn(s.T, cv, __fmul_rn(ra, __fmaf_rn(s.bdot, -1.0f, s.tfva)));
+    s.bdot = __fmaf_rn(w.fac, cv, s.bdot);
+    w.g = __fmul_rn(araw_g, v_alpha);
     if constexpr (kEwa) {
         w.w1 = w.g; // the moments are sums of g {x, y, x^2, xy, y^2}: the conic's chain rule runs per Gaussian
-        w.w2 = f2_bc(0.0f);
+        w.w2 = 0.0f;
     } else {
-        const f2 gr = f2_mul(w.g, rD);
-        w.w1 = f2_mul(gr, f2_bc(kLn2));
-        w.w2 = f2_mul(f2_mul(gr, f2_bc(-kLn2)), f2_mul(e.Ns, rD));
+        w.w1 = __fmul_rn(__fmul_rn(w.g, rD), kLn2);
+        w.w2 = __fmul_rn(-w.w1, __fmul_rn(e.Ns, rD));
     }
     return w;
 }
 
-// Shuffle reduction: the 16 registers of the event, lanes 16..31 pre-swapped (see MomentSlot).
-template <bool kEwa = false>
-__device__ __forceinline__ void event_registers(const BwdState &s, const EventWeights &w, const PairEval2 &e, f2 x, f2 y,
-                                                bool hi16, float (&R)[16]) {
-    if constexpr (kEwa) {
-        // nine live slots (g, g x, g y, g xx, g xy, g yy, colour): lanes 16..31 hold them in the swapped registers
-        const float gs = f2_sum(w.g);
-        const float m1 = f2_sum(f2_mul(w.g, x)), m2 = f2_sum(f2_mul(w.g, y));
-        const float m3 = f2_sum(f2_mul(w.g, e.xx)), m4 = f2_sum(f2_mul(w.g, e.xy)), m5 = f2_sum(f2_mul(w.g, e.yy));
-        R[0] = hi16 ? 0.0f : gs; R[8] = hi16 ? gs : 0.0f;
-        R[1] = hi16 ? 0.0f : m1; R[9] = hi16 ? m1 : 0.0f;
-        R[2] = hi16 ? 0.0f : m2; R[10] = hi16 ? m2 : 0.0f;
-        R[3] = hi16 ? 0.0f : m3; R[11] = hi16 ? m3 : 0.0f;
-        R[4] = hi16 ? 0.0f : m4; R[12] = hi16 ? m4 : 0.0f;
-        R[5] = hi16 ? 0.0f : m5; R[13] = hi16 ? m5 : 0.0f;
-        R[6] = f2_sum(f2_mul(w.fac, s.vA)); R[14] = f2_sum(f2_mul(w.fac, s.vB));
-        R[7] = f2_sum(f2_mul(w.fac, s.vC)); R[15] = f2_sum(f2_mul(w.fac, s.vD));
-        return;
+// The five moments  sum w {x, y, x^2, xy, y^2}  and  sum w  of one weight over a thread's pixels.  On a
+// shared column they follow from  S0 = sum w, S1 = sum w y, S2 = sum w y^2  and the column's x; a general
+// camera gives every pixel its own x.  These sums need not match any other kernel bit for bit: plain
+// float arithmetic, which the compiler contracts.
+template <bool kSharedX, int kPix>
+__device__ __forceinline__ void weight_moments(const float (&w)[kPix], const PixEval (&e)[kPix],
+                                               const ColTerms (&c)[kSharedX ? 1 : kPix], float (&m)[6]) {
+    float S0 = 0.0f, S1 = 0.0f, S2 = 0.0f, X1 = 0.0f, XX = 0.0f, XY = 0.0f;
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        const float wy = w[i] * e[i].y;
+        S0 += w[i];
+        S1 += wy;
+        S2 += wy * e[i].y;
+        if constexpr (!kSharedX) {
+            const float wx = w[i] * c[i].x;
+            X1 += wx;
+            XX += wx * c[i].x;
+            XY += wx * e[i].y;
+        }
     }
-    const f2 wA = hi16 ? w.w2 : w.w1, wB = hi16 ? w.w1 : w.w2;
-    const float gs = f2_sum(w.g), w2s = f2_sum(w.w2);
-    R[0] = hi16 ? w2s : gs;
-    R[8] = hi16 ? gs : w2s;
-    R[1] = f2_sum(f2_mul(wA, x)); R[2] = f2_sum(f2_mul(wA, y));
-    R[3] = f2_sum(f2_mul(wA, e.xx)); R[4] = f2_sum(f2_mul(wA, e.xy)); R[5] = f2_sum(f2_mul(wA, e.yy));
-    R[9] = f2_sum(f2_mul(wB, x)); R[10] = f2_sum(f2_mul(wB, y));
-    R[11] = f2_sum(f2_mul(wB, e.xx)); R[12] = f2_sum(f2_mul(wB, e.xy)); R[13] = f2_sum(f2_mul(wB, e.yy));
-    R[6] = f2_sum(f2_mul(w.fac, s.vA)); R[14] = f2_sum(f2_mul(w.fac, s.vB));
-    R[7] = f2_sum(f2_mul(w.fac, s.vC)); R[15] = f2_sum(f2_mul(w.fac, s.vD));
+    if constexpr (kSharedX) {
+        X1 = c[0].x * S0;
+        XX = c[0].xx * S0;
+        XY = c[0].x * S1;
+    }
+    m[0] = S0; m[1] = X1; m[2] = S1; m[3] = XX; m[4] = XY; m[5] = S2;
 }
 
-template <bool kGeneral, bool kEwa = false>
-__global__ void __launch_bounds__(kTileThreads) raster_bwd_kernel(const TileParams p,
-                                                                   const float *__restrict__ render_alphas,
-                                                                   const int32_t *__restrict__ last_ids,
-                                                                   const float *__restrict__ v_render_colors,
-                                                                   const float *__restrict__ v_render_alphas,
-                                                                   float *__restrict__ moments) {
+// The 16 registers of an event for the warp reduction, lanes 16..31 pre-swapped (see MomentSlot):
+// lane L < 16 holds slot i in R[i], lane L >= 16 holds slot i ^ 8.
+template <bool kEwa, bool kSharedX, int kPix>
+__device__ __forceinline__ void event_registers(const BwdPixel (&s)[kPix], const EventWeights (&w)[kPix],
+                                                const PixEval (&e)[kPix], const ColTerms (&c)[kSharedX ? 1 : kPix],
+                                                bool hi16, float (&R)[16]) {
+    float mA[6], mB[6], gs;
+    if constexpr (kEwa) {
+        // six live slots (g, g x, g y, g xx, g xy, g yy): lanes 16..31 hold them in the swapped registers
+        float g[kPix];
+#pragma unroll
+        for (int i = 0; i < kPix; ++i) g[i] = w[i].g;
+        float m[6];
+        weight_moments<kSharedX, kPix>(g, e, c, m);
+        gs = m[0];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) { mA[k] = hi16 ? 0.0f : m[k]; mB[k] = hi16 ? m[k] : 0.0f; }
+    } else {
+        // weight A fills slots 1..5 (w1 on lanes 0..15, w2 on lanes 16..31), weight B slots 9..13
+        float wA[kPix], wB[kPix];
+        gs = 0.0f;
+#pragma unroll
+        for (int i = 0; i < kPix; ++i) {
+            wA[i] = hi16 ? w[i].w2 : w[i].w1;
+            wB[i] = hi16 ? w[i].w1 : w[i].w2;
+            gs += w[i].g;
+        }
+        weight_moments<kSharedX, kPix>(wA, e, c, mA);
+        weight_moments<kSharedX, kPix>(wB, e, c, mB);
+    }
+    R[0] = hi16 ? mA[0] : gs; // slot 0 = sum g, slot 8 = sum w2
+    R[8] = hi16 ? gs : mB[0];
+#pragma unroll
+    for (int k = 1; k < 6; ++k) { R[k] = mA[k]; R[k + 8] = mB[k]; }
+    float cr = 0.0f, cg = 0.0f, cb = 0.0f;
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        cr += w[i].fac * s[i].vr;
+        cg += w[i].fac * s[i].vg;
+        cb += w[i].fac * s[i].vb;
+    }
+    R[6] = hi16 ? cg : cr; R[14] = hi16 ? cr : cg; // slots kS_CR / kS_CG
+    R[7] = hi16 ? 0.0f : cb; R[15] = hi16 ? cb : 0.0f; // slots kS_CB / kS_PAD
+}
+
+template <bool kGeneral, bool kEwa, int kPix>
+__global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams p,
+                                                                const float *__restrict__ render_alphas,
+                                                                const int32_t *__restrict__ last_ids,
+                                                                const float *__restrict__ v_render_colors,
+                                                                const float *__restrict__ v_render_alphas,
+                                                                float *__restrict__ moments) {
     // Three stages; a stage is filled through its "full" mbarrier (TMA byte count) and released through its "empty"
     // mbarrier (one arrival per warp): no CTA-wide barrier in the loop, a warp with nothing to do in a batch runs ahead
-    // of its neighbours instead of waiting at a two-stage / __syncthreads ring.
-    constexpr int kRing = 3;
+    // of its neighbour instead of waiting at a two-stage / __syncthreads ring.
+    constexpr int kBatch = 256 / kPix, kWarps = 256 / kPix / 32, kRing = 3;
     __shared__ __align__(128) GaussRec s_rec[kRing][kBatch];
     __shared__ __align__(8) uint64_t s_full[kRing];
     __shared__ __align__(8) uint64_t s_empty[kRing];
-    __shared__ int32_t s_warp_max[kTileThreads / 32];
+    __shared__ int32_t s_warp_max[kWarps];
     __shared__ CamModel s_cm;
     const uint32_t tile_id = blockIdx.x;
     if (p.masks != nullptr && !p.masks[tile_id]) return; // Bwd.cu:84-86
     const uint32_t tile_y = tile_id / p.tile_w, tile_x = tile_id % p.tile_w;
-    const PixelMap pm = pixel_map(tile_x, tile_y, p.W, p.H);
+    const PixelMap<kPix> pm = pixel_map<kPix>(tile_x, tile_y, p.W, p.H);
     const uint32_t tid = threadIdx.x;
     const bool hi16 = (tid & 16) != 0;
 
@@ -425,11 +499,20 @@ __global__ void __launch_bounds__(kTileThreads) raster_bwd_kernel(const TilePara
     float bg[3] = {0.f, 0.f, 0.f};
     if (p.backgrounds) { bg[0] = p.backgrounds[0]; bg[1] = p.backgrounds[1]; bg[2] = p.backgrounds[2]; }
 
-    struct PixelIn { float T, vr, vg, vb, tfva; int32_t last; };
-    auto load_pixel = [&](bool in, uint32_t y) {
-        PixelIn r;
-        if (in) {
-            const size_t pix = (size_t)y * p.W + pm.x;
+    if constexpr (kGeneral) {
+        if (tid == 0) tile_cam_build(p, s_cm);
+        __syncthreads();
+    }
+    const PixelCoords<kPix> pc = pixel_coords<kGeneral, kPix>(pm, tile_x, tile_y, &s_cm);
+    BwdPixel s[kPix];
+    int32_t wmax = -1;
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        BwdPixel &r = s[i];
+        r.in = pm.in[i] && pc.ok[i];
+        r.bdot = 0.0f;
+        if (r.in) {
+            const size_t pix = (size_t)pm.y[i] * p.W + pm.x;
             const float Tf = 1.0f - render_alphas[pix];
             r.T = Tf;
             r.last = last_ids[pix];
@@ -441,40 +524,19 @@ __global__ void __launch_bounds__(kTileThreads) raster_bwd_kernel(const TilePara
         } else {
             r.T = 1.f; r.last = -1; r.vr = r.vg = r.vb = 0.f; r.tfva = 0.f;
         }
-        return r;
-    };
-    if constexpr (kGeneral) {
-        if (tid == 0) tile_cam_build(p, s_cm);
-        __syncthreads();
+        wmax = max(wmax, r.last);
     }
-    const PixelCoords pc = pixel_coords<kGeneral>(p, pm, tile_x, tile_y, &s_cm);
-    BwdState s;
-    s.in0 = pm.in0 && pc.ok0;
-    s.in1 = pm.in1 && pc.ok1;
-    {
-        const PixelIn a = load_pixel(s.in0, pm.y0), b = load_pixel(s.in1, pm.y1);
-        s.T = f2_make(a.T, b.T);
-        s.bdot = f2_bc(0.0f);
-        s.tfva = f2_make(a.tfva, b.tfva);
-        s.vr = f2_make(a.vr, b.vr); s.vg = f2_make(a.vg, b.vg); s.vb = f2_make(a.vb, b.vb);
-        s.vA = hi16 ? s.vg : s.vr;
-        s.vB = hi16 ? s.vr : s.vg;
-        s.vC = hi16 ? f2_bc(0.0f) : s.vb;
-        s.vD = hi16 ? s.vb : f2_bc(0.0f);
-        s.last0 = a.last; s.last1 = b.last;
-    }
-    const f2 PX = f2_make(pc.px0, pc.px1), PY = f2_make(pc.py0, pc.py1);
     // CTA-wide newest contributor: nothing behind it can receive gradient
-    int32_t wmax = __reduce_max_sync(0xffffffffu, max(s.last0, s.last1));
+    wmax = __reduce_max_sync(0xffffffffu, wmax);
     if ((tid & 31) == 0) s_warp_max[tid >> 5] = wmax;
     if (tid == 0) {
-        for (int st = 0; st < kRing; ++st) { mbar_init(&s_full[st], 1); mbar_init(&s_empty[st], kTileThreads / 32); }
+        for (int st = 0; st < kRing; ++st) { mbar_init(&s_full[st], 1); mbar_init(&s_empty[st], kWarps); }
         mbar_fence_init();
     }
     __syncthreads();
     int32_t hi = s_warp_max[0];
 #pragma unroll
-    for (int w = 1; w < kTileThreads / 32; ++w) hi = max(hi, s_warp_max[w]);
+    for (int w = 1; w < kWarps; ++w) hi = max(hi, s_warp_max[w]);
     hi = min(hi, range_end - 1);
     const int32_t total = hi - range_start + 1;
     if (total <= 0) return;
@@ -522,15 +584,27 @@ __global__ void __launch_bounds__(kTileThreads) raster_bwd_kernel(const TilePara
             cmask &= cmask - 1;
             const int32_t idx = top - t;
             const float4 q0 = rec4[t * 4], q1 = rec4[t * 4 + 1], q2 = rec4[t * 4 + 2];
-            const f2 x = f2_add(PX, f2_bc(-q0.x)), y = f2_add(PY, f2_bc(-q0.y));
-            const PairEval2 e = pair_eval2<kEwa>(q0, q1, q2, x, y);
-            const bool p0 = e.pass0 && s.in0 && idx <= s.last0;
-            const bool p1 = e.pass1 && s.in1 && idx <= s.last1;
-            if (!__any_sync(0xffffffffu, p0 || p1)) continue;
+            ColTerms c[kGeneral ? kPix : 1];
+            PixEval e[kPix];
+            eval_pixels<kEwa, !kGeneral, kPix>(q0, q1, q2, pc.px, pc.py, c, e);
+            bool pass[kPix], any = false;
+#pragma unroll
+            for (int i = 0; i < kPix; ++i) {
+                pass[i] = e[i].pass && s[i].in && idx <= s[i].last;
+                any = any || pass[i];
+            }
+            if (!__any_sync(0xffffffffu, any)) continue;
             const float4 q3 = rec4[t * 4 + 3];
-            const EventWeights w = bwd_weights<kEwa>(s, e, p0, p1, q2.z, q3.x, q3.y, q3.z);
+            // A record often covers only part of the warp's 16 rows: a pixel index that no lane passes gets zero
+            // weights and keeps its state, exactly what bwd_weights would give it, without the MUFU work.
+            EventWeights w[kPix];
+#pragma unroll
+            for (int i = 0; i < kPix; ++i) {
+                if (__any_sync(0xffffffffu, pass[i])) w[i] = bwd_weights<kEwa>(s[i], e[i], pass[i], q2.z, q3.x, q3.y, q3.z);
+                else w[i] = EventWeights{0.0f, 0.0f, 0.0f, 0.0f};
+            }
             float R[16];
-            event_registers<kEwa>(s, w, e, x, y, hi16, R);
+            event_registers<kEwa, !kGeneral, kPix>(s, w, e, c, hi16, R);
             butterfly16_preswapped(R);
             if ((tid & 1) == 0) {
                 const uint32_t slot = (tid & 31) >> 1;
@@ -646,23 +720,52 @@ static int launch_fwd(const TileParams &p, const GsbCamera *cam, float *renders,
     {
         ProfScope ps("raster_fwd", s);
         if (general_camera(cam))
-            raster_fwd_kernel<true><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, renders, alphas, last_ids);
+            raster_fwd_kernel<true><<<p.tile_w * p.tile_h, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
         else
-            raster_fwd_kernel<false><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, renders, alphas, last_ids);
+            raster_fwd_kernel<false><<<p.tile_w * p.tile_h, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
+}
+// Four pixels per thread pay an event's reduction and REDs once per 128 pixels, but give a tile only two warps.  An
+// image with fewer tiles than the GPU holds such CTAs at once (256x256: 256 tiles, against 132 SMs x 14 CTAs on an
+// H100 SXM) runs two pixels per thread instead: four warps per tile to hide latency with.
+static uint32_t bwd_wide_min_tiles() {
+    // immutable after the first call (C++11 thread-safe initialisation)
+    static const uint32_t n = [] {
+        int sms = 132, per_sm = 14, dev = 0;
+        if (cudaGetDevice(&dev) == cudaSuccess) {
+            int v = 0;
+            if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sms = v;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, raster_bwd_kernel<false, false, kBwdPix>, 256 / kBwdPix,
+                                                              0) == cudaSuccess && v > 0)
+                per_sm = v;
+        }
+        return (uint32_t)(sms * per_sm);
+    }();
+    return n;
+}
+template <bool kGeneral, bool kEwa>
+static void launch_bwd_kernel(const TileParams &p, const float *render_alphas, const int32_t *last_ids,
+                              const float *v_render_colors, const float *v_render_alphas, float *moments,
+                              cudaStream_t s) {
+    const uint32_t tiles = p.tile_w * p.tile_h;
+    if (tiles >= bwd_wide_min_tiles())
+        raster_bwd_kernel<kGeneral, kEwa, kBwdPix><<<tiles, 256 / kBwdPix, 0, s>>>(p, render_alphas, last_ids,
+                                                                                  v_render_colors, v_render_alphas,
+                                                                                  moments);
+    else
+        raster_bwd_kernel<kGeneral, kEwa, kBwdPixSmall><<<tiles, 256 / kBwdPixSmall, 0, s>>>(
+            p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments);
 }
 static int launch_bwd(const TileParams &p, const GsbCamera *cam, const float *render_alphas, const int32_t *last_ids,
                       const float *v_render_colors, const float *v_render_alphas, float *moments, cudaStream_t s) {
     {
         ProfScope ps("raster_bwd", s);
         if (general_camera(cam))
-            raster_bwd_kernel<true><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, render_alphas, last_ids,
-                                                                                v_render_colors, v_render_alphas, moments);
+            launch_bwd_kernel<true, false>(p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, s);
         else
-            raster_bwd_kernel<false><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, render_alphas, last_ids,
-                                                                                 v_render_colors, v_render_alphas, moments);
+            launch_bwd_kernel<false, false>(p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, s);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
@@ -685,7 +788,7 @@ int raster_ewa_fwd(uint32_t cap, const GaussRec *recs, uint32_t W, uint32_t H, c
     fill_ewa(p, cap, W, H, recs, tile_offsets, flatten_ids);
     {
         ProfScope ps("ewa_blend_fwd", s);
-        raster_fwd_kernel<false, true><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, image, alpha, last_ids);
+        raster_fwd_kernel<false, true><<<p.tile_w * p.tile_h, kFwdThreads, 0, s>>>(p, image, alpha, last_ids);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
@@ -697,8 +800,7 @@ int raster_ewa_bwd(uint32_t cap, const GaussRec *recs, uint32_t W, uint32_t H, c
     fill_ewa(p, cap, W, H, recs, tile_offsets, flatten_ids);
     {
         ProfScope ps("ewa_blend_bwd", s);
-        raster_bwd_kernel<false, true><<<p.tile_w * p.tile_h, kTileThreads, 0, s>>>(p, alpha, last_ids, grad_image,
-                                                                                   grad_alpha, moments);
+        launch_bwd_kernel<false, true>(p, alpha, last_ids, grad_image, grad_alpha, moments, s);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;

@@ -290,38 +290,67 @@ __device__ __forceinline__ void finalize_gaussian(const CamConst &cam, const flo
     }
 }
 
-// Per-pair evaluation, shared VERBATIM by the forward and backward kernels (explicitly rounded
-// operations: the two kernels must agree bit-for-bit on which pairs pass the alpha test), for a
-// thread's two pixels at once on packed fp32 pairs (lo = pixel 0, hi = pixel 1):
+// Per-pixel evaluation, shared VERBATIM by the forward and backward kernels (explicitly rounded
+// operations: the two kernels must agree bit-for-bit on which pairs pass the alpha test):
 //   Ns = n0 x^2 + n1 xy + n2 y^2          (pre-scaled by -1/2 log2 e / d0)
 //   Ds = 1 + d1 x + d2 y + d3 x^2 + d4 xy + d5 y^2
 //   pass <=> Ns >= tau Ds                  (MUFU-free rejection, tau carries a safety margin)
-struct PairEval2 {
-    f2 Ns, Ds;
-    f2 xx, xy, yy;
-    bool pass0, pass1;
-};
+// written as polynomials in y whose coefficients depend on x only:
+//   Ns = a + y (b + n2 y),  a = n0 x^2,  b = n1 x
+//   Ds = P + y (Q + d5 y),  P = 1 + d1 x + d3 x^2,  Q = d2 + d4 x
+// A thread's pixels lie in one column on a pinhole (and EWA) camera, so it computes the column terms
+// once per record and two FFMAs per polynomial per pixel.  A pixel's value does not depend on how many
+// pixels share its column terms: each pixel runs the same operations in the same order.
 // kEwa: the record is a pure 2-D conic (SURVEY.md 8 f4, gsb_fastgs.cu): Ds == 1, no denominator arithmetic.
+struct ColTerms {
+    float x, xx, a, b, P, Q;
+};
 template <bool kEwa = false>
-__device__ __forceinline__ PairEval2 pair_eval2(const float4 q0, const float4 q1, const float4 q2, f2 x, f2 y) {
-    PairEval2 r;
-    r.xx = f2_mul(x, x); r.xy = f2_mul(x, y); r.yy = f2_mul(y, y);
-    r.Ns = f2_fma(f2_bc(q1.x), r.yy, f2_fma(f2_bc(q0.w), r.xy, f2_mul(f2_bc(q0.z), r.xx)));
-    f2 t;
+__device__ __forceinline__ ColTerms col_terms(const float4 q0, const float4 q1, const float4 q2, float px) {
+    ColTerms c;
+    c.x = __fadd_rn(px, -q0.x);
+    c.xx = __fmul_rn(c.x, c.x);
+    c.a = __fmul_rn(q0.z, c.xx);
+    c.b = __fmul_rn(q0.w, c.x);
     if constexpr (kEwa) {
-        r.Ds = f2_bc(1.0f);
-        t = f2_add(r.Ns, f2_bc(-q2.w)); // Ns >= tau
+        c.P = 1.0f; c.Q = 0.0f;
     } else {
-        f2 D = f2_fma(f2_bc(q1.y), x, f2_bc(1.0f));
-        D = f2_fma(f2_bc(q1.z), y, D);
-        D = f2_fma(f2_bc(q1.w), r.xx, D);
-        D = f2_fma(f2_bc(q2.x), r.xy, D);
-        r.Ds = f2_fma(f2_bc(q2.y), r.yy, D);
-        t = f2_fma(f2_bc(-q2.w), r.Ds, r.Ns); // Ns >= tau * Ds
+        c.P = __fmaf_rn(q1.w, c.xx, __fmaf_rn(q1.y, c.x, 1.0f));
+        c.Q = __fmaf_rn(q2.x, c.x, q1.z);
     }
-    r.pass0 = f2_lo(t) >= 0.0f;
-    r.pass1 = f2_hi(t) >= 0.0f;
-    return r;
+    return c;
+}
+struct PixEval {
+    float y, Ns, Ds;
+    bool pass;
+};
+template <bool kEwa = false>
+__device__ __forceinline__ PixEval pix_eval(const ColTerms &c, const float4 q0, const float4 q1, const float4 q2,
+                                            float py) {
+    PixEval e;
+    e.y = __fadd_rn(py, -q0.y);
+    e.Ns = __fmaf_rn(e.y, __fmaf_rn(q1.x, e.y, c.b), c.a);
+    if constexpr (kEwa) {
+        e.Ds = 1.0f;
+        e.pass = e.Ns >= q2.w; // Ns >= tau
+    } else {
+        e.Ds = __fmaf_rn(e.y, __fmaf_rn(q2.y, e.y, c.Q), c.P);
+        e.pass = __fmaf_rn(-q2.w, e.Ds, e.Ns) >= 0.0f; // Ns >= tau * Ds
+    }
+    return e;
+}
+// All kPix pixels of a thread against one record.  kSharedX: the pixels share one column (px[0]) and one
+// set of column terms c[0]; otherwise (general camera: each pixel's undistorted x differs) c[i] is pixel i's.
+template <bool kEwa, bool kSharedX, int kPix>
+__device__ __forceinline__ void eval_pixels(const float4 q0, const float4 q1, const float4 q2, const float (&px)[kPix],
+                                            const float (&py)[kPix], ColTerms (&c)[kSharedX ? 1 : kPix],
+                                            PixEval (&e)[kPix]) {
+    if constexpr (kSharedX) c[0] = col_terms<kEwa>(q0, q1, q2, px[0]);
+#pragma unroll
+    for (int i = 0; i < kPix; ++i) {
+        if constexpr (!kSharedX) c[i] = col_terms<kEwa>(q0, q1, q2, px[i]);
+        e[i] = pix_eval<kEwa>(c[kSharedX ? 0 : i], q0, q1, q2, py[i]);
+    }
 }
 // Warp-level culling: can ANY pixel of the warp's block, whose (undistorted) pixel coordinates lie
 // in the box [bx0, bx1] x [by0, by1], pass the rejection test of this record?  The pass region {Ns - tau Ds >= 0} is the interior of an
@@ -383,13 +412,6 @@ __device__ __forceinline__ bool block_may_pass(const float4 q0, const float4 q1,
         }
     }
     return fmax >= -0.02f;
-}
-
-// alpha_raw = opac * exp(power) = 2^(Ns/Ds + lop)
-template <bool kEwa = false>
-__device__ __forceinline__ float pair_alpha_raw(float Ns, float Ds, float lop) {
-    if constexpr (kEwa) return fast_ex2(__fadd_rn(Ns, lop));
-    return fast_ex2(__fmaf_rn(Ns, fast_rcp(Ds), lop));
 }
 
 } // namespace gsb
