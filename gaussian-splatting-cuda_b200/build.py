@@ -43,9 +43,10 @@ CUDA_SOURCES = [
     ("gsb_loss.cu", []),
     ("gsb_optim.cu", []),
     ("gsb_fastgs.cu", []),
+    ("gsb_bilagrid.cu", []),
 ]
 CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh"]
-SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
+SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
 
 
 def _run(cmd: list[str], verbose: bool) -> str:
@@ -127,7 +128,8 @@ def build_shim(verbose: bool = False, force: bool = False) -> str:
     for i in [os.path.join(INC, "gsplat"), os.path.join(INC, "fastgs"), INC] + tinc + [cuda_inc]:
         incs += ["-I", i]
     hdrs = [os.path.join(INC, "gsb200.h")] + [os.path.join(INC, "gsplat", h) for h in ("Ops.h", "FusedOps.h", "Common.h", "Cameras.h")] + \
-        [os.path.join(INC, "fastgs", "rasterization_api.h"), os.path.join(INC, "fastgs", "rasterization_ext.h")]
+        [os.path.join(INC, "fastgs", "rasterization_api.h"), os.path.join(INC, "fastgs", "rasterization_ext.h"),
+         os.path.join(INC, "kernels", "bilateral_grid.cuh")]
     def compile_one(src: str) -> str:
         sp = os.path.join(SHIM, src)
         op = os.path.join(OBJ, "shim_" + src.replace(".cpp", ".o"))

@@ -63,6 +63,8 @@ struct LossSmem {
 static_assert(sizeof(float2) * kSH * kTP <= sizeof(float2) * (kIH + 1) * kSP, "g01 alias");
 static_assert(sizeof(float) * kSH * kTP <= sizeof(float) * (kIH + 1) * kSP, "g2 alias");
 
+// NoClamp (GSB_LOSS_NO_CLAMP): the renders enter as they are and every pixel passes the gradient
+template <bool NoClamp>
 __global__ void __launch_bounds__(kLossThreads, 3) ssim_l1_kernel(const LossParams p) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     LossSmem &S = *reinterpret_cast<LossSmem *>(s_raw);
@@ -100,11 +102,11 @@ __global__ void __launch_bounds__(kLossThreads, 3) ssim_l1_kernel(const LossPara
                     float X = 0.f, Y = 0.f;
                     if (row_ok && gx >= 0 && gx < W) {
                         const float raw = rrow[gx * rstep];
-                        X = fminf(fmaxf(raw, 0.f), 1.f);
+                        X = NoClamp ? raw : fminf(fmaxf(raw, 0.f), 1.f);
                         Y = trow[gx * tstep];
                         // the tile's own pixels remember whether the clamp was active (dLoss/d(render) = 0 there)
                         const int tr = r - 2 * kHalo, tq = q - 2 * kHalo;
-                        if (tr >= 0 && tr < kTH && tq >= 0 && tq < kTW) s_pass[tr][tq] = (raw >= 0.f && raw <= 1.f) ? 1 : 0;
+                        if (tr >= 0 && tr < kTH && tq >= 0 && tq < kTW) s_pass[tr][tq] = (NoClamp || (raw >= 0.f && raw <= 1.f)) ? 1 : 0;
                     }
                     S.xy[r][q] = make_float2(X, Y);
                 }
@@ -322,10 +324,11 @@ extern "C" int gsb_ssim_l1(uint32_t image_width, uint32_t image_height, const fl
     p.y_lo = crop ? 5 : 0; p.y_hi = crop ? image_height - 5 : image_height;
     p.x_lo = crop ? 5 : 0; p.x_hi = crop ? image_width - 5 : image_width;
     const dim3 grid((image_width + kTW - 1) / kTW, (image_height + kTH - 1) / kTH);
-    GSB_CUDA_TRY(cudaFuncSetAttribute(ssim_l1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LossSmem)));
+    auto kernel = (target_chw & GSB_LOSS_NO_CLAMP) ? ssim_l1_kernel<true> : ssim_l1_kernel<false>;
+    GSB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LossSmem)));
     {
         ProfScope ps(v_renders ? "ssim_l1_bwd" : "ssim_l1_fwd", s);
-        ssim_l1_kernel<<<grid, kLossThreads, sizeof(LossSmem), s>>>(p);
+        kernel<<<grid, kLossThreads, sizeof(LossSmem), s>>>(p);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;

@@ -211,8 +211,9 @@ rasterize_from_world_fused_bwd(const at::Tensor means, const at::Tensor sh0, con
     return std::make_tuple(v_means, v_sh0, v_shN, v_scaling, v_rotation, v_opacity);
 }
 
-GSB_EXPORT std::tuple<at::Tensor, at::Tensor> photometric_loss_fused(const at::Tensor renders, const at::Tensor target,
-                                                                     const float lambda_dssim, const bool compute_grad) {
+namespace {
+std::tuple<at::Tensor, at::Tensor> photometric_loss_impl(const at::Tensor &renders, const at::Tensor &target,
+                                                         const float lambda_dssim, const bool compute_grad, const int flags) {
     const c10::cuda::CUDAGuard guard(renders.device());
     CHECK_F32(renders);
     CHECK_F32(target);
@@ -230,11 +231,24 @@ GSB_EXPORT std::tuple<at::Tensor, at::Tensor> photometric_loss_fused(const at::T
     if (compute_grad) v_renders = at::empty_like(renders);
     at::Tensor ws = at::empty({(int64_t)gsb_ssim_l1_workspace()}, renders.options().dtype(at::kByte));
     gsb_check(gsb_ssim_l1((uint32_t)W, (uint32_t)H, renders.data_ptr<float>(), target.data_ptr<float>(),
-                          (chw ? GSB_LOSS_TARGET_CHW : 0) | (r_chw ? GSB_LOSS_RENDERS_CHW : 0),
+                          (chw ? GSB_LOSS_TARGET_CHW : 0) | (r_chw ? GSB_LOSS_RENDERS_CHW : 0) | flags,
                           lambda_dssim, 1.0f, compute_grad ? v_renders.data_ptr<float>() : nullptr, stats.data_ptr<float>(),
                           ws.data_ptr(), (size_t)ws.numel(), cur_stream()),
               "photometric_loss_fused");
     return std::make_tuple(stats, v_renders);
+}
+} // namespace
+
+GSB_EXPORT std::tuple<at::Tensor, at::Tensor> photometric_loss_fused(const at::Tensor renders, const at::Tensor target,
+                                                                     const float lambda_dssim, const bool compute_grad) {
+    return photometric_loss_impl(renders, target, lambda_dssim, compute_grad, 0);
+}
+
+GSB_EXPORT std::tuple<at::Tensor, at::Tensor> photometric_loss_fused_unclamped(const at::Tensor renders,
+                                                                               const at::Tensor target,
+                                                                               const float lambda_dssim,
+                                                                               const bool compute_grad) {
+    return photometric_loss_impl(renders, target, lambda_dssim, compute_grad, GSB_LOSS_NO_CLAMP);
 }
 
 GSB_EXPORT void fused_adam_step(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,

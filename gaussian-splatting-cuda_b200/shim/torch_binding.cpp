@@ -185,6 +185,14 @@ std::tuple<Tensor, Tensor> loss_fused(const Tensor &renders, const Tensor &targe
     return std::make_tuple(std::get<0>(r), v);
 }
 
+std::tuple<Tensor, Tensor> loss_fused_unclamped(const Tensor &renders, const Tensor &target, double lambda_dssim,
+                                                bool compute_grad) {
+    auto r = gsplat::photometric_loss_fused_unclamped(renders, target, (float)lambda_dssim, compute_grad);
+    Tensor v = std::get<1>(r);
+    if (!v.defined()) v = at::empty({0}, renders.options());
+    return std::make_tuple(std::get<0>(r), v);
+}
+
 void adam_step(std::vector<Tensor> params, std::vector<Tensor> grads, std::vector<Tensor> exp_avg,
                std::vector<Tensor> exp_avg_sq, std::vector<double> lr, double beta1, double beta2, double eps,
                std::vector<int64_t> step_counts) {
@@ -233,6 +241,7 @@ TORCH_LIBRARY(gsplat_b200, m) {
           "Tensor v_render_colors, Tensor v_render_alphas) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)",
           &fused_bwd);
     m.def("photometric_loss_fused", &loss_fused);
+    m.def("photometric_loss_fused_unclamped", &loss_fused_unclamped);
     m.def("fused_adam_step(Tensor(a!)[] params, Tensor[] grads, Tensor(b!)[] exp_avg, Tensor(c!)[] exp_avg_sq, float[] lr, "
           "float beta1, float beta2, float eps, int[] step_counts) -> ()",
           &adam_step);

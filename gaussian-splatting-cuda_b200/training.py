@@ -6,6 +6,9 @@
                      iterations), all groups stepped by ONE kernel launch (gsb_adam_step)
   TrainStep          render (extended operator on the raw tensors) -> loss -> backward -> Adam [-> MCMC noise], with
                      the intersection buffer sized from a capacity so that the iteration has no host read-back
+  bilateral_grid     optional (SURVEY.md 8 f5, trainer.cpp:662-665,698-705,758-762): render -> slice through the
+                     image's grid -> unclamped loss -> + weight * TV of all grids -> backward -> one Adam launch for the
+                     Gaussians and the grids (lr from the warm-up/exponential schedule, eps 1e-15)
 
 Everything that computes lives behind the C ABI; this file only orders the calls, like the reference's trainer does."""
 from __future__ import annotations
@@ -16,6 +19,7 @@ from dataclasses import dataclass, field
 import torch
 
 from . import _product_ns, load, rasterize_fused
+from .bilateral import BilateralGrid, WarmupExponentialLR
 
 
 class _PhotometricLoss(torch.autograd.Function):
@@ -31,6 +35,27 @@ class _PhotometricLoss(torch.autograd.Function):
     def backward(ctx, g_loss, _g_stats):
         (v,) = ctx.saved_tensors
         return (v * g_loss if v.numel() else None), None, None
+
+
+class _PhotometricLossUnclamped(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, renders, target, lambda_dssim):
+        stats, v = _product_ns().photometric_loss_fused_unclamped(renders.detach().contiguous(), target.contiguous(),
+                                                                  float(lambda_dssim), renders.requires_grad)
+        ctx.save_for_backward(v)
+        ctx.mark_non_differentiable(stats)
+        return stats[0], stats
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_stats):
+        (v,) = ctx.saved_tensors
+        return (v * g_loss if v.numel() else None), None, None
+
+
+def photometric_loss_unclamped(renders, target, lambda_dssim: float = 0.2):
+    """photometric_loss on an image used as it is (no clamp, no clamp mask): the loss of a bilateral-grid output."""
+    load()
+    return _PhotometricLossUnclamped.apply(renders, target, lambda_dssim)
 
 
 def photometric_loss(renders, target, lambda_dssim: float = 0.2):
@@ -74,7 +99,9 @@ class FusedAdam:
         self.exp_avg_sq = {k: torch.zeros_like(v) for k, v in params.items()}
         self.steps = {k: 0 for k in params}
 
-    def step(self, iteration: int):
+    def step(self, iteration: int, extra: tuple | None = None):
+        """extra: one more group (param, grad, exp_avg, exp_avg_sq, lr, step count, (beta1, beta2, eps)), stepped by the
+        same launch when its hyperparameters are the Gaussians' and by a second launch otherwise."""
         names, counts = [], []
         for k in PARAM_GROUPS:
             p = self.params[k]
@@ -85,17 +112,86 @@ class FusedAdam:
                 continue
             names.append(k)
             counts.append(self.steps[k])
-        if names:
+        if names and extra is None:
             with torch.no_grad():
                 _product_ns().fused_adam_step([self.params[k] for k in names], [self.params[k].grad for k in names],
                                               [self.exp_avg[k] for k in names], [self.exp_avg_sq[k] for k in names],
                                               [self.lr[PARAM_GROUPS.index(k)] for k in names], self.cfg.beta1,
                                               self.cfg.beta2, self.cfg.eps, counts)
+        elif extra is not None:
+            p, g, m, v, lr, t, hyper = extra
+            c = self.cfg
+            ns = _product_ns()
+            with torch.no_grad():
+                if hyper == (c.beta1, c.beta2, c.eps):
+                    ns.fused_adam_step([self.params[k] for k in names] + [p], [self.params[k].grad for k in names] + [g],
+                                       [self.exp_avg[k] for k in names] + [m], [self.exp_avg_sq[k] for k in names] + [v],
+                                       [self.lr[PARAM_GROUPS.index(k)] for k in names] + [lr], c.beta1, c.beta2, c.eps,
+                                       counts + [t])
+                else:
+                    if names:
+                        ns.fused_adam_step([self.params[k] for k in names], [self.params[k].grad for k in names],
+                                           [self.exp_avg[k] for k in names], [self.exp_avg_sq[k] for k in names],
+                                           [self.lr[PARAM_GROUPS.index(k)] for k in names], c.beta1, c.beta2, c.eps, counts)
+                    ns.fused_adam_step([p], [g], [m], [v], [lr], hyper[0], hyper[1], hyper[2], [t])
         self.lr[0] *= self.gamma
 
     def zero_grad(self):
         for p in self.params.values():
             p.grad = None
+
+
+class _GridState:
+    """What the training iteration keeps for the bilateral grids: the device image index, the TV weight as a device
+    scalar, the grids' Adam moments and step count, and their learning-rate schedule (trainer.cpp:66-101)."""
+
+    # the grids' own torch::optim::Adam (trainer.cpp:81-83): default betas, eps 1e-15 -- independent of the Gaussians'
+    beta1, beta2, eps = 0.9, 0.999, 1e-15
+
+    def __init__(self, grid: BilateralGrid, lr: float, tv_weight: float, iterations: int):
+        g = grid.grids
+        self.grid = grid
+        self.sched = WarmupExponentialLR(lr, iterations)
+        self.exp_avg, self.exp_avg_sq = torch.zeros_like(g), torch.zeros_like(g)
+        self.steps = 0
+        self.idx = torch.zeros(1, dtype=torch.int32, device=g.device)
+        self.weight = torch.full((1,), float(tv_weight), dtype=torch.float32, device=g.device)
+
+    def set_image(self, image_idx) -> None:
+        if image_idx is None or not 0 <= int(image_idx) < self.grid.num_images:
+            raise ValueError(f"a training step with a bilateral grid needs an image index in [0, {self.grid.num_images})")
+        self.idx.fill_(int(image_idx))  # a kernel argument: no host buffer to race with
+
+    def tv(self):
+        """(TV loss of all grids, weight * its gradient): the buffer the slice backward then adds into."""
+        return _product_ns().bilagrid_tv(self.grid.grids.detach(), self.weight, True)
+
+    def adam_group(self):
+        """The grids' Adam group for this step; advances the schedule (bilateral_grid_scheduler_->step())."""
+        self.steps += 1
+        g = self.grid.grids
+        group = (g.detach(), g.grad, self.exp_avg, self.exp_avg_sq, self.sched.lr, self.steps,
+                 (self.beta1, self.beta2, self.eps))
+        self.sched.step()
+        return group
+
+
+class _SliceIntoGrad(torch.autograd.Function):
+    """Slice for the training step: the backward ADDS the grid gradient into v_grids (the TV gradient of all grids)
+    and returns the gradient of the unclamped render only."""
+
+    @staticmethod
+    def forward(ctx, image, grids, image_idx, v_grids, chw):
+        image = image.detach().contiguous()
+        ctx.save_for_backward(image, grids, image_idx, v_grids)
+        ctx.chw = chw
+        return _product_ns().bilagrid_slice(grids, image, image_idx, chw)
+
+    @staticmethod
+    def backward(ctx, v_out):
+        image, grids, image_idx, v_grids = ctx.saved_tensors
+        return _product_ns().bilagrid_slice_backward(grids, image, image_idx, v_out.contiguous(), v_grids, ctx.chw), \
+            None, None, None, None
 
 
 @dataclass
@@ -111,17 +207,40 @@ class TrainStep:
     capacity: int = 0                    # intersections the buffers are sized for; 0 = size exactly (one read-back)
     iteration: int = 0
     last: dict = field(default_factory=dict)
+    bilateral_grid: BilateralGrid | None = None  # use_bilateral_grid: the iteration needs image_idx
+    bilateral_grid_lr: float = 2e-3
+    tv_loss_weight: float = 10.0                 # mcmc_optimization_params.json (default_optimization_params.json: 5)
+    grid_state: _GridState | None = None         # created on first use
 
-    def __call__(self, viewmat, K, target, background=None):
+    def _grid(self) -> _GridState:
+        if self.grid_state is None:
+            its = self.optimizer.cfg.iterations if self.optimizer is not None else AdamConfig().iterations
+            self.grid_state = _GridState(self.bilateral_grid, self.bilateral_grid_lr, self.tv_loss_weight, its)
+        return self.grid_state
+
+    def __call__(self, viewmat, K, target, background=None, image_idx=None):
         P = self.params
         self.iteration += 1
         out = rasterize_fused(P["means"], P["sh0"], P["shN"], P["scaling_raw"], P["rotation_raw"], P["opacity_raw"],
                               self.sh_degree, viewmat, K, self.width, self.height, bg_color=background,
                               isect_capacity=self.capacity)
-        loss, stats = photometric_loss(out.render_colors, target, self.lambda_dssim)
-        loss.backward()
+        extra = None
+        if self.bilateral_grid is None:
+            loss, stats = photometric_loss(out.render_colors, target, self.lambda_dssim)
+            loss.backward()
+        else:
+            G = self._grid()
+            G.set_image(image_idx)
+            tv, v_grids = G.tv()
+            sliced = _SliceIntoGrad.apply(out.render_colors, G.grid.grids.detach(), G.idx, v_grids, False)
+            loss, stats = photometric_loss_unclamped(sliced, target, self.lambda_dssim)
+            loss.backward()
+            G.grid.grids.grad = v_grids
+            loss = loss.detach() + G.weight[0] * tv  # the trainer's loss_value includes the TV term
         if self.optimizer is not None:
-            self.optimizer.step(self.iteration)
+            if self.bilateral_grid is not None:
+                extra = self.grid_state.adam_group()
+            self.optimizer.step(self.iteration, extra)
             if self.mcmc_noise_lr > 0.0:
                 with torch.no_grad():
                     noise = torch.randn_like(P["means"])
@@ -129,6 +248,8 @@ class TrainStep:
                                             P["rotation_raw"].detach(), noise, P["means"].detach(),
                                             self.mcmc_noise_lr * self.optimizer.lr[0])
             self.optimizer.zero_grad()
+        if self.bilateral_grid is not None:
+            self.bilateral_grid.grids.grad = None
         self.last = {"n_isects": out.n_isects, "stats": stats}
         return loss
 
@@ -155,7 +276,8 @@ class GraphedTrainStep:
     (pinned -> device, on the replay stream) and reads the loss back when it wants to."""
 
     def __init__(self, params: dict, sh_degree: int, width: int, height: int, cfg: AdamConfig | None = None,
-                 lambda_dssim: float = 0.2, capacity_slack: float = 1.25):
+                 lambda_dssim: float = 0.2, capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None,
+                 bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0):
         load()
         self.params, self.sh_degree, self.W, self.H = params, int(sh_degree), int(width), int(height)
         self.lambda_dssim = float(lambda_dssim)
@@ -166,8 +288,13 @@ class GraphedTrainStep:
         self.static = {"viewmat": torch.zeros((1, 4, 4), device=dev), "K": torch.zeros((1, 3, 3), device=dev),
                        "background": torch.zeros((1, 3), device=dev),
                        "target": torch.zeros((3, self.H, self.W), device=dev)}
-        self.dyn = torch.zeros((len(PARAM_GROUPS), 4), device=dev)
-        self.dyn_host = torch.zeros((len(PARAM_GROUPS), 4)).pin_memory()
+        # with a bilateral grid, its image index is a device input and its Adam scalars are one more row of `dyn`
+        self.bilateral_grid = bilateral_grid
+        self.grid_state = (_GridState(bilateral_grid, bilateral_grid_lr, tv_loss_weight, self.opt.cfg.iterations)
+                           if bilateral_grid is not None else None)
+        n_rows = len(PARAM_GROUPS) + (1 if bilateral_grid is not None else 0)
+        self.dyn = torch.zeros((n_rows, 4), device=dev)
+        self.dyn_host = torch.zeros((n_rows, 4)).pin_memory()
         self.graph = None
         self.loss = None
         self.stats = None
@@ -180,17 +307,48 @@ class GraphedTrainStep:
         out = rasterize_fused(P["means"], P["sh0"], P["shN"], P["scaling_raw"], P["rotation_raw"], P["opacity_raw"],
                               self.sh_degree, S["viewmat"], S["K"], self.W, self.H, bg_color=S["background"],
                               isect_capacity=self.capacity)
-        loss, stats = photometric_loss(out.render_colors, S["target"], self.lambda_dssim)
+        if self.grid_state is None:
+            loss, stats = photometric_loss(out.render_colors, S["target"], self.lambda_dssim)
+            loss.backward()
+            self._adam()
+            return loss, stats, out.n_isects
+        G = self.grid_state
+        tv, v_grids = G.tv()
+        sliced = _SliceIntoGrad.apply(out.render_colors, G.grid.grids.detach(), G.idx, v_grids, False)
+        loss, stats = photometric_loss_unclamped(sliced, S["target"], self.lambda_dssim)
         loss.backward()
+        self._adam(v_grids)
+        return loss.detach() + G.weight[0] * tv, stats, out.n_isects
+
+    def _adam(self, v_grids=None):
+        """One launch for the Gaussians' groups (and the grids' after them), scalars from `dyn`."""
+        P = self.params
         names = [k for k in PARAM_GROUPS if P[k].numel() > 0]
         with torch.no_grad():
-            _product_ns().fused_adam_step_dynamic([P[k] for k in names], [P[k].grad for k in names],
-                                                  [self.opt.exp_avg[k] for k in names],
-                                                  [self.opt.exp_avg_sq[k] for k in names],
-                                                  self.dyn[[PARAM_GROUPS.index(k) for k in names]].contiguous()
-                                                  if len(names) != len(PARAM_GROUPS) else self.dyn,
-                                                  self.opt.cfg.beta1, self.opt.cfg.beta2, self.opt.cfg.eps)
-        return loss, stats, out.n_isects
+            if v_grids is None:
+                _product_ns().fused_adam_step_dynamic([P[k] for k in names], [P[k].grad for k in names],
+                                                      [self.opt.exp_avg[k] for k in names],
+                                                      [self.opt.exp_avg_sq[k] for k in names],
+                                                      self.dyn[[PARAM_GROUPS.index(k) for k in names]].contiguous()
+                                                      if len(names) != len(PARAM_GROUPS) else self.dyn,
+                                                      self.opt.cfg.beta1, self.opt.cfg.beta2, self.opt.cfg.eps)
+                return
+            G, c, ns = self.grid_state, self.opt.cfg, _product_ns()
+            rows = [PARAM_GROUPS.index(k) for k in names]
+            if (G.beta1, G.beta2, G.eps) == (c.beta1, c.beta2, c.eps):  # one launch for all groups
+                rows.append(len(PARAM_GROUPS))
+                ns.fused_adam_step_dynamic([P[k] for k in names] + [G.grid.grids.detach()],
+                                           [P[k].grad for k in names] + [v_grids],
+                                           [self.opt.exp_avg[k] for k in names] + [G.exp_avg],
+                                           [self.opt.exp_avg_sq[k] for k in names] + [G.exp_avg_sq],
+                                           self.dyn[rows].contiguous() if len(rows) != self.dyn.shape[0] else self.dyn,
+                                           c.beta1, c.beta2, c.eps)
+                return
+            ns.fused_adam_step_dynamic([P[k] for k in names], [P[k].grad for k in names],
+                                       [self.opt.exp_avg[k] for k in names], [self.opt.exp_avg_sq[k] for k in names],
+                                       self.dyn[rows].contiguous(), c.beta1, c.beta2, c.eps)
+            ns.fused_adam_step_dynamic([G.grid.grids.detach()], [v_grids], [G.exp_avg], [G.exp_avg_sq],
+                                       self.dyn[len(PARAM_GROUPS):].contiguous(), G.beta1, G.beta2, G.eps)
 
     def _set_inputs(self, viewmat, K, target, background):
         S = self.static
@@ -211,12 +369,22 @@ class GraphedTrainStep:
             self.dyn_host[i, 1] = 1.0 / (1.0 - o.cfg.beta1 ** t)
             self.dyn_host[i, 2] = 1.0 / math.sqrt(1.0 - o.cfg.beta2 ** t)
             self.dyn_host[i, 3] = enabled
+        if self.grid_state is not None:  # the grids' group: torch.optim.Adam's bias corrections, the scheduled lr
+            G, i = self.grid_state, len(PARAM_GROUPS)
+            G.steps += 1
+            self.dyn_host[i, 0] = G.sched.lr
+            self.dyn_host[i, 1] = 1.0 / (1.0 - G.beta1 ** G.steps)
+            self.dyn_host[i, 2] = 1.0 / math.sqrt(1.0 - G.beta2 ** G.steps)
+            self.dyn_host[i, 3] = 1.0
+            G.sched.step()
         self.dyn.copy_(self.dyn_host, non_blocking=True)
         o.lr[0] *= o.gamma
 
-    def capture(self, viewmat, K, target, background=None):
+    def capture(self, viewmat, K, target, background=None, image_idx=None):
         """Sizes the intersection capacity with one exact render, warms up and captures the graph."""
         self._set_inputs(viewmat, K, target, background)
+        if self.grid_state is not None:
+            self.grid_state.set_image(image_idx)
         with torch.no_grad():
             P, S = self.params, self.static
             out = rasterize_fused(P["means"], P["sh0"], P["shN"], P["scaling_raw"], P["rotation_raw"], P["opacity_raw"],
@@ -239,11 +407,13 @@ class GraphedTrainStep:
             self.loss, self.stats, self.n_isects = self._body()
         return n
 
-    def __call__(self, viewmat, K, target, background=None):
+    def __call__(self, viewmat, K, target, background=None, image_idx=None):
         if self.graph is None:
-            self.capture(viewmat, K, target, background)
+            self.capture(viewmat, K, target, background, image_idx)
         self.iteration += 1
         self._set_inputs(viewmat, K, target, background)
+        if self.grid_state is not None:
+            self.grid_state.set_image(image_idx)
         self._set_scalars()
         self.graph.replay()
         return self.loss
@@ -270,6 +440,17 @@ class FastGsTrainStep:
     capacity: int = 0                     # > 0: instance buffer sized from it, no host read-back (rasterization_ext.h)
     iteration: int = 0
     last: dict = field(default_factory=dict)
+    bilateral_grid: BilateralGrid | None = None  # use_bilateral_grid: the iteration needs image_idx
+    bilateral_grid_lr: float = 2e-3
+    tv_loss_weight: float = 10.0
+    grid_state: _GridState | None = None         # created on first use
+    index_on_device: bool = False                # the graphed wrapper refreshes grid_state.idx itself before each replay
+
+    def _grid(self) -> _GridState:
+        if self.grid_state is None:
+            its = self.optimizer.cfg.iterations if self.optimizer is not None else AdamConfig().iterations
+            self.grid_state = _GridState(self.bilateral_grid, self.bilateral_grid_lr, self.tv_loss_weight, its)
+        return self.grid_state
 
     def size_capacity(self, w2c, settings, slack: float = 1.25):
         """One exact (synchronising) forward sizes the instance capacity for the following iterations."""
@@ -283,18 +464,34 @@ class FastGsTrainStep:
         self.capacity = int(n * slack) + 1024
         return n
 
-    def __call__(self, w2c, settings, target, background=None, densification_info=None):
+    def __call__(self, w2c, settings, target, background=None, densification_info=None, image_idx=None):
         from . import fastgs as fg
         be = self.backend or fg.default_backend()
         P = self.params
         self.iteration += 1
+        G = None
+        if self.bilateral_grid is not None:
+            G = self._grid()
+            if not self.index_on_device:
+                G.set_image(image_idx)
         with torch.no_grad():
             opac = P["opacity_raw"].reshape(-1, 1)
             image, alpha, ctx = be.forward(P["means"], P["scaling_raw"], P["rotation_raw"], opac, P["sh0"], P["shN"], w2c, settings,
                                            capacity=self.capacity)
             final = image + (1.0 - alpha) * background.reshape(3, 1, 1) if background is not None else image
-            stats, v_final = _product_ns().photometric_loss_fused(final.contiguous(), target.contiguous(),
-                                                                  float(self.lambda_dssim), True)
+            if G is None:
+                stats, v_final = _product_ns().photometric_loss_fused(final.contiguous(), target.contiguous(),
+                                                                      float(self.lambda_dssim), True)
+            else:  # slice -> unclamped loss -> slice backward (adds into the TV gradient of all grids)
+                ns = _product_ns()
+                final = final.contiguous()
+                tv, v_grids = G.tv()
+                grids = G.grid.grids.detach()
+                sliced = ns.bilagrid_slice(grids, final, G.idx, True)
+                stats, v_sliced = ns.photometric_loss_fused_unclamped(sliced, target.contiguous(), float(self.lambda_dssim),
+                                                                      True)
+                v_final = ns.bilagrid_slice_backward(grids, final, G.idx, v_sliced, v_grids, True)
+                G.grid.grids.grad = v_grids
             v_alpha = (-(v_final * background.reshape(3, 1, 1)).sum(0, keepdim=True) if background is not None
                        else torch.zeros_like(alpha))
             g = be.backward(ctx, v_final, v_alpha.contiguous(), image, alpha, P["means"], P["scaling_raw"], P["rotation_raw"],
@@ -302,11 +499,13 @@ class FastGsTrainStep:
             for k, gk in zip(("means", "scaling_raw", "rotation_raw", "opacity_raw", "sh0", "shN"), g[:6]):
                 P[k].grad = gk.reshape(P[k].shape)
         if self.optimizer is not None:
-            self.optimizer.step(self.iteration)
+            self.optimizer.step(self.iteration, G.adam_group() if G is not None else None)
             self.optimizer.zero_grad()
+            if G is not None:
+                G.grid.grids.grad = None
         # capacity mode: the count is a device tensor (compare it with the capacity when convenient)
         self.last = {"n_instances": ctx.get("n_instances_dev", int(ctx["ints"][1])), "stats": stats}
-        return stats[0]
+        return stats[0] if G is None else stats[0] + G.weight[0] * tv
 
 
 class GraphedFastGsTrainStep(GraphedTrainStep):
@@ -316,8 +515,10 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
     size are launch arguments and therefore fixed per captured graph (one graph per camera resolution)."""
 
     def __init__(self, params: dict, sh_degree: int, settings, cfg: AdamConfig | None = None, lambda_dssim: float = 0.2,
-                 capacity_slack: float = 1.25):
-        super().__init__(params, sh_degree, settings.width, settings.height, cfg, lambda_dssim, capacity_slack)
+                 capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None, bilateral_grid_lr: float = 2e-3,
+                 tv_loss_weight: float = 10.0):
+        super().__init__(params, sh_degree, settings.width, settings.height, cfg, lambda_dssim, capacity_slack,
+                         bilateral_grid, bilateral_grid_lr, tv_loss_weight)
         from . import fastgs as fg
         dev = self.dev
         self.static = {"w2c": torch.zeros((4, 4), device=dev), "campos": torch.zeros((3,), device=dev),
@@ -328,20 +529,14 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
                                           near_plane=settings.near_plane, far_plane=settings.far_plane)
         self.be = fg.default_backend()
         self.step = FastGsTrainStep(params, sh_degree, settings.width, settings.height, lambda_dssim, optimizer=None,
-                                    backend=self.be)
+                                    backend=self.be, bilateral_grid=bilateral_grid, grid_state=self.grid_state,
+                                    index_on_device=True)
 
     def _body(self):
         P, S = self.params, self.static
         self.step.capacity = self.capacity
         loss = self.step(S["w2c"], self.settings, S["target"], S["background"])
-        names = [k for k in PARAM_GROUPS if P[k].numel() > 0]
-        with torch.no_grad():
-            _product_ns().fused_adam_step_dynamic([P[k] for k in names], [P[k].grad for k in names],
-                                                  [self.opt.exp_avg[k] for k in names],
-                                                  [self.opt.exp_avg_sq[k] for k in names],
-                                                  self.dyn[[PARAM_GROUPS.index(k) for k in names]].contiguous()
-                                                  if len(names) != len(PARAM_GROUPS) else self.dyn,
-                                                  self.opt.cfg.beta1, self.opt.cfg.beta2, self.opt.cfg.eps)
+        self._adam(self.grid_state.grid.grids.grad if self.grid_state is not None else None)
         return loss, self.step.last["stats"], self.step.last["n_instances"]
 
     def _set_inputs(self, w2c, cam_position, target, background):
@@ -352,8 +547,10 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
         if background is not None:
             S["background"].copy_(background.reshape(3), non_blocking=True)
 
-    def capture(self, w2c, cam_position, target, background=None):
+    def capture(self, w2c, cam_position, target, background=None, image_idx=None):
         self._set_inputs(w2c, cam_position, target, background)
+        if self.grid_state is not None:
+            self.grid_state.set_image(image_idx)
         self.step.capacity = 0
         n = self.step.size_capacity(self.static["w2c"], self.settings, self.slack)
         self.capacity = self.step.capacity
@@ -369,11 +566,13 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
             self.loss, self.stats, self.n_isects = self._body()
         return n
 
-    def __call__(self, w2c, cam_position, target, background=None):
+    def __call__(self, w2c, cam_position, target, background=None, image_idx=None):
         if self.graph is None:
-            self.capture(w2c, cam_position, target, background)
+            self.capture(w2c, cam_position, target, background, image_idx)
         self.iteration += 1
         self._set_inputs(w2c, cam_position, target, background)
+        if self.grid_state is not None:
+            self.grid_state.set_image(image_idx)
         self._set_scalars()
         self.graph.replay()
         return self.loss

@@ -309,8 +309,10 @@ GSB_API int gsb_fused_back(const GsbSplatRaw *splats, const GsbCamera *cam, uint
  * target_chw is a bit set: GSB_LOSS_TARGET_CHW (1) = target is [3,H,W]; GSB_LOSS_RENDERS_CHW (2) = renders AND v_renders
  * are [3,H,W] planes (the fastgs path's image, SURVEY.md 8 f4).
  * v_renders (laid out like renders) = grad_scale * dLoss/d(renders) including the clamp mask, or NULL to evaluate only.
- * loss_out: DEVICE float[3] = (loss, l1 mean, ssim mean).  workspace: gsb_ssim_l1_workspace() bytes, 256-aligned. */
-enum { GSB_LOSS_TARGET_CHW = 1, GSB_LOSS_RENDERS_CHW = 2 };
+ * loss_out: DEVICE float[3] = (loss, l1 mean, ssim mean).  workspace: gsb_ssim_l1_workspace() bytes, 256-aligned.
+ * GSB_LOSS_NO_CLAMP (4): the renders are used as they are -- no clamp and no clamp mask -- as the reference's loss
+ * treats an image that went through the bilateral grid (trainer.cpp:662-665 -> 103-126). */
+enum { GSB_LOSS_TARGET_CHW = 1, GSB_LOSS_RENDERS_CHW = 2, GSB_LOSS_NO_CLAMP = 4 };
 GSB_API size_t gsb_ssim_l1_workspace(void);
 GSB_API int gsb_ssim_l1(uint32_t image_width, uint32_t image_height, const float *renders, const float *target,
                         int target_chw, float lambda_dssim, float grad_scale, float *v_renders /*nullable*/,
@@ -378,6 +380,32 @@ GSB_API int gsb_fastgs_backward(uint32_t N, const float *means, const float *sca
                                 float *grad_scales_raw, float *grad_rotations_raw /*16-byte aligned*/,
                                 float *grad_opacities_raw, float *grad_sh0, float *grad_shN, float *grad_w2c /*nullable*/,
                                 float *densification_info /*nullable*/, gsb_stream_t stream);
+
+/* ---- SURVEY.md 8(f5): the bilateral grid of the training iteration (appearance correction per image) ---------------
+ * src/training/components/bilateral_grid.cpp:94-127 and src/training/kernels/bilateral_grid_{forward,backward,tv}.cu.
+ * grids: [n_images, 12, grid_l, grid_h, grid_w] float32 (grid_w = bilateral_grid_X, grid_h = _Y, grid_l = _W, the
+ * guidance depth).  image_idx: DEVICE int32 scalar selecting the grid (NULL = 0), so a captured CUDA graph can slice a
+ * different image per replay; an index outside [0, n_images) writes NaN into the output / input gradient.
+ * The image is [H,W,3] or, with GSB_BILAGRID_CHW in `layout`, [3,H,W]; the output / gradients have the input's layout.
+ * The slice clamps the input to [0,1] first (bilateral_grid.cpp:110); the backward returns the gradient with respect
+ * to the UNCLAMPED input (zero where input < 0 or > 1) and ADDS the grid gradient into v_grids (only image_idx's grid
+ * is touched).  Image width and height must be >= 2 (the grid coordinates divide by width-1 and height-1).
+ * gsb_bilagrid_tv: loss_out (DEVICE float) = (1 / (12 n_images)) * sum over (n, c) of the means of the squared
+ * neighbour differences along x, y and z; if v_grids is non-NULL it is WRITTEN in full with *grad_weight (DEVICE float,
+ * NULL = 1) times the loss's gradient.  Deterministic; workspace: gsb_bilagrid_tv_workspace() bytes, 256-aligned. */
+enum { GSB_BILAGRID_CHW = 1 };
+GSB_API int gsb_bilagrid_slice_fwd(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l, uint32_t n_images,
+                                   const float *grids, const int32_t *image_idx /*DEVICE, nullable*/, uint32_t image_width,
+                                   uint32_t image_height, int layout, const float *input, float *output,
+                                   gsb_stream_t stream);
+GSB_API int gsb_bilagrid_slice_bwd(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l, uint32_t n_images,
+                                   const float *grids, const int32_t *image_idx /*DEVICE, nullable*/, uint32_t image_width,
+                                   uint32_t image_height, int layout, const float *input, const float *v_output,
+                                   float *v_grids /*added into*/, float *v_input, gsb_stream_t stream);
+GSB_API size_t gsb_bilagrid_tv_workspace(void);
+GSB_API int gsb_bilagrid_tv(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l, uint32_t n_images, const float *grids,
+                            const float *grad_weight /*DEVICE, nullable*/, float *loss_out, float *v_grids /*nullable*/,
+                            void *workspace, size_t workspace_bytes, gsb_stream_t stream);
 
 /* ---- link-surface ops used by the densification strategies -------------------------
  * gsplat::quats_to_rotmats (Ops.h:46-48, QuatToRotmatCUDA.cu:14-39): [N,4] -> [N,3,3] */

@@ -77,6 +77,11 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
 std::tuple<at::Tensor, at::Tensor> photometric_loss_fused(const at::Tensor renders, const at::Tensor target,
                                                           const float lambda_dssim, const bool compute_grad);
 
+// SURVEY.md 8 (f5): the same loss on an image used as it is -- no clamp, no clamp mask -- as the reference computes it
+// on the output of the bilateral grid (trainer.cpp:662-665 -> 103-126).
+std::tuple<at::Tensor, at::Tensor> photometric_loss_fused_unclamped(const at::Tensor renders, const at::Tensor target,
+                                                                    const float lambda_dssim, const bool compute_grad);
+
 // SURVEY.md 8 (f3): one Adam step over all parameter groups in one launch (fastgs/optimizer/include/adam_kernels.cuh:13-36,
 // src/training/optimizers/fused_adam.cpp:22-95).  step_counts are the per-group counts AFTER the increment.
 void fused_adam_step(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,
