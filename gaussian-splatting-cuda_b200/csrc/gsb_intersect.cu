@@ -23,12 +23,11 @@
 //   5. column scan over (tile, chunk): M[p][t] becomes the first output slot of chunk p in tile t;
 //                the tile offsets (a6) fall out of the same scan.
 //   -- host reads n_isects, allocates the outputs --
-//   6. scatter   the same pass again, each intersection taking the next slot of its (chunk, tile) group: 4 bytes
-//                written per intersection DIRECTLY into the final range of its group, nothing read back.
-//   7. repair    groups with more than one member (1.35 intersections per group at config B) are put into depth
-//                order in place; the 64-bit keys, when the caller wants them, are written by a coalesced pass.
-// Chunks are in depth order and groups are ordered by (depth bits, index) inside: every tile's list is ordered by
-// (depth, index) -- the same permutation as the reference's single 46-bit sort, ties included.
+//   6. place     the same pass again, each intersection taking the next slot of its (chunk, tile) group in run order:
+//                4 bytes written per intersection DIRECTLY to its final position, nothing read back; the 64-bit keys,
+//                when the caller wants them, are written by a coalesced pass.
+// Chunks are in depth order and groups are filled in run order, which is (depth bits, index) order: every tile's list
+// is ordered by (depth, index) -- the same permutation as the reference's single 46-bit sort, ties included.
 #include "gsb_devsort.cuh"
 #include "gsb_ewa.cuh"
 
@@ -299,18 +298,20 @@ __global__ void __launch_bounds__(kSortThreads) runs_build_kernel(SortCtl *__res
     }
 }
 
-// ---- steps 4, 6 and 7: per-chunk tile counters, placement, order repair -----------------------------------------------
+// ---- steps 4 and 6: per-chunk tile counters, ordered placement ------------------------------------------------
 // The runs (Gaussians with tiles, in depth order) are cut into P chunks of about I / P intersections each, at run
 // boundaries.  One CTA per chunk keeps one counter per tile in shared memory.
-//   hist     every intersection of the chunk does an atomicAdd on its tile's counter -> M[p][tile] (any order);
-//   scatter  the counters start at the chunk's first slot in each tile (column scan of M) and every intersection
-//            takes the next slot of its tile: the (chunk, tile) GROUPS land in their final ranges, but the order
-//            INSIDE a group is the order the atomics retired in;
-//   repair   every group with more than one member is put into depth order: groups of up to 16 by an insertion sort
-//            on (depth bits, index) -- a Gaussian appears at most once per group, so this is the run order -- larger
-//            groups by REGENERATION: a warp walks the chunk's runs in order and re-emits those that cover the tile.
-// With P = 888 chunks and 8160 tiles a group holds 1.35 intersections on average at config B, so the repair touches
-// a fraction of the data; nothing in these three kernels is serial.
+//   hist   every intersection of the chunk does an atomicAdd on its tile's counter -> M[p][tile] (any order);
+//   place  the counters start at the chunk's first slot in each tile (column scan of M) and every intersection takes
+//          the next slot of its tile IN RUN ORDER, so each (chunk, tile) group lands in its final range already in
+//          (depth bits, index) order: the runs are in that order (stable depth sort) and a run covers a tile at most
+//          once.
+// How place keeps run order without a CTA-wide handshake: warp w owns the tile rows y with y % 8 == w (of every
+// camera), so no two warps share a counter and a tile's order is decided inside ONE warp.  Every warp walks all the
+// chunk's runs, 32 per step (one per lane), and expands only its rows of their boxes; the expanded intersections are
+// laid out flat in run order and taken 32 per round, so the lanes of a round are in run order and rounds follow
+// each other.  Inside a round every lane takes a slot with a shared atomic; when a tile has several members in the
+// round (the atomic tells), the members are re-ranked by lane.
 struct BinArgs {
     RunTable rt;
     const SortCtl *ctl;
@@ -324,10 +325,10 @@ struct BinArgs {
     uint32_t *chunk_run;  // [P + 1] first run of every chunk (written by hist)
     int32_t *flatten_ids;
     uint32_t cap;         // capacity of flatten_ids (>= n_isects unless the caller under-allocated)
-    const float *depths;  // [C * N] (scatter pass: order repair)
 };
 
 constexpr int kBinThreads = 256;
+constexpr uint32_t kBinWarps = kBinThreads / 32; // place: warp w owns the tile rows y % kBinWarps == w
 
 // first r in [0, n_runs) with end[r] > s (exists: s < end[n_runs - 1]); one probe per lane and round
 __device__ __forceinline__ uint32_t first_run_after(const uint32_t *__restrict__ end, uint32_t n_runs, uint32_t s) {
@@ -354,214 +355,28 @@ __device__ __forceinline__ uint32_t chunk_first_run(const BinArgs &a, uint32_t p
     return first_run_after(a.rt.end, n_runs, s);
 }
 
-// Order repair of the (chunk, tile) groups: one lane per group, a warp for the large ones.  Called by all 32 lanes
-// of a warp, each with its own group: chunk p, global tile t, slots [start, start + c) of flatten_ids.
-constexpr int kLaneSortMax = 16;  // groups of up to this many members are sorted by their own lane
-constexpr int kWarpSortMax = 128; // larger groups of up to this many members are rank-sorted by a warp
-
-// groups of two to four members: a 4-element sorting network in registers
-__device__ __forceinline__ void repair_small(const BinArgs &a, const float *__restrict__ depths, uint32_t start,
-                                             uint32_t c) {
-    if (c >= 2 && c <= 4) {
-        // the common case (a group holds 1.35 intersections on average): a 4-element sorting network in registers
-        uint32_t id0 = (uint32_t)a.flatten_ids[start], id1 = (uint32_t)a.flatten_ids[start + 1];
-        uint32_t id2 = c > 2 ? (uint32_t)a.flatten_ids[start + 2] : 0xffffffffu;
-        uint32_t id3 = c > 3 ? (uint32_t)a.flatten_ids[start + 3] : 0xffffffffu;
-        uint32_t k0 = __float_as_uint(depths[id0]), k1 = __float_as_uint(depths[id1]);
-        uint32_t k2 = c > 2 ? __float_as_uint(depths[id2]) : 0xffffffffu;
-        uint32_t k3 = c > 3 ? __float_as_uint(depths[id3]) : 0xffffffffu;
-        bool moved = false;
-        auto cswap = [&](uint32_t &ka, uint32_t &ia, uint32_t &kb, uint32_t &ib) {
-            if (kb < ka || (kb == ka && ib < ia)) {
-                const uint32_t tk = ka, ti = ia;
-                ka = kb; ia = ib; kb = tk; ib = ti;
-                moved = true;
-            }
-        };
-        cswap(k0, id0, k1, id1); cswap(k2, id2, k3, id3); cswap(k0, id0, k2, id2); cswap(k1, id1, k3, id3);
-        cswap(k1, id1, k2, id2);
-        if (moved) {
-            a.flatten_ids[start] = (int32_t)id0;
-            a.flatten_ids[start + 1] = (int32_t)id1;
-            if (c > 2) a.flatten_ids[start + 2] = (int32_t)id2;
-            if (c > 3) a.flatten_ids[start + 3] = (int32_t)id3;
-        }
-    }
-}
-
-template <bool kFilter>
-__device__ __forceinline__ void repair_groups(const BinArgs &a, const float *__restrict__ depths, uint32_t p,
-                                              uint32_t t, uint32_t start, uint32_t c) {
-    const uint32_t lane = threadIdx.x & 31;
-    if (c >= 2 && c <= 4) {
-        repair_small(a, depths, start, c);
-    } else if (c > 4 && c <= 8) {
-        // up to eight: Batcher's odd-even merge network (19 comparators) in registers, padding with +inf keys
-        uint32_t id[8], k[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            id[e] = (uint32_t)e < c ? (uint32_t)a.flatten_ids[start + e] : 0xffffffffu;
-            k[e] = (uint32_t)e < c ? __float_as_uint(depths[id[e]]) : 0xffffffffu;
-        }
-        bool moved = false;
-        auto cs = [&](int i, int j) {
-            if (k[j] < k[i] || (k[j] == k[i] && id[j] < id[i])) {
-                const uint32_t tk = k[i], ti = id[i];
-                k[i] = k[j]; id[i] = id[j]; k[j] = tk; id[j] = ti;
-                moved = true;
-            }
-        };
-        cs(0, 1); cs(2, 3); cs(4, 5); cs(6, 7);
-        cs(0, 2); cs(1, 3); cs(4, 6); cs(5, 7);
-        cs(1, 2); cs(5, 6);
-        cs(0, 4); cs(1, 5); cs(2, 6); cs(3, 7);
-        cs(2, 4); cs(3, 5);
-        cs(1, 2); cs(3, 4); cs(5, 6);
-        if (moved) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if ((uint32_t)e < c) a.flatten_ids[start + e] = (int32_t)id[e];
-        }
-    } else if (c > 8 && c <= (uint32_t)kLaneSortMax) {
-        // nine to sixteen: insertion sort on (depth bits, index) in local memory, one group per lane (32 groups of a warp
-        // keep their gathers in flight together; handing these to the warp-wide sort below serialises them: measured)
-        uint32_t ids[kLaneSortMax], keys[kLaneSortMax];
-        for (uint32_t k = 0; k < c; ++k) {
-            ids[k] = (uint32_t)a.flatten_ids[start + k];
-            keys[k] = __float_as_uint(depths[ids[k]]);
-        }
-        bool moved = false;
-        for (uint32_t k = 1; k < c; ++k) {
-            const uint32_t kk = keys[k], ki = ids[k];
-            uint32_t j = k;
-            while (j > 0 && (kk < keys[j - 1] || (kk == keys[j - 1] && ki < ids[j - 1]))) {
-                keys[j] = keys[j - 1]; ids[j] = ids[j - 1];
-                --j;
-                moved = true;
-            }
-            keys[j] = kk; ids[j] = ki;
-        }
-        if (moved)
-            for (uint32_t k = 0; k < c; ++k) a.flatten_ids[start + k] = (int32_t)ids[k];
-    }
-    // kLaneSortMax + 1 to kWarpSortMax members: the whole warp sorts one group at a time by RANK -- every lane holds up to four
-    // (depth bits, index) pairs, counts for each how many of the group's pairs are smaller (pairs are distinct: a Gaussian
-    // appears once per group) and stores it at that position.  O(c^2 / 32) shuffles per group, no dependent re-walk of the
-    // chunk: what keeps the pass flat when depth and screen position correlate and (chunk, tile) groups grow (a camera
-    // looking along the slab's diagonal: groups of 20..60; the per-group re-walk below took 0.83 ms there, DESIGN.md 4.3).
-    uint32_t mid = __ballot_sync(0xffffffffu, c > (uint32_t)kLaneSortMax && c <= (uint32_t)kWarpSortMax);
-    while (mid) {
-        const int src = __ffs(mid) - 1;
-        mid &= mid - 1;
-        const uint32_t gstart = __shfl_sync(0xffffffffu, start, src), gc = __shfl_sync(0xffffffffu, c, src);
-        const uint32_t slots = (gc + 31u) >> 5; // elements per lane, <= kWarpSortMax / 32
-        if (slots == 1u) { // up to 32 members (the common case of this path): one pair per lane, gc shuffle rounds
-            const uint32_t id1 = lane < gc ? (uint32_t)a.flatten_ids[gstart + lane] : 0xffffffffu;
-            const uint32_t k1 = lane < gc ? __float_as_uint(depths[id1]) : 0xffffffffu;
-            uint32_t r1 = 0;
-            for (uint32_t l = 0; l < gc; ++l) {
-                const uint32_t ko = __shfl_sync(0xffffffffu, k1, l), io = __shfl_sync(0xffffffffu, id1, l);
-                r1 += (ko < k1 || (ko == k1 && io < id1)) ? 1u : 0u;
-            }
-            if (lane < gc && r1 != lane) a.flatten_ids[gstart + r1] = (int32_t)id1;
-            continue;
-        }
-        uint32_t id[kWarpSortMax / 32], k[kWarpSortMax / 32];
-#pragma unroll
-        for (int e = 0; e < kWarpSortMax / 32; ++e) {
-            const uint32_t j = (uint32_t)e * 32u + lane;
-            id[e] = j < gc ? (uint32_t)a.flatten_ids[gstart + j] : 0xffffffffu;
-        }
-#pragma unroll
-        for (int e = 0; e < kWarpSortMax / 32; ++e) k[e] = id[e] != 0xffffffffu ? __float_as_uint(depths[id[e]]) : 0xffffffffu;
-        uint32_t rank[kWarpSortMax / 32];
-#pragma unroll
-        for (int e = 0; e < kWarpSortMax / 32; ++e) rank[e] = 0;
-#pragma unroll
-        for (int f = 0; f < kWarpSortMax / 32; ++f) {
-            if ((uint32_t)f < slots) { // warp-uniform
-                for (int l = 0; l < 32; ++l) {
-                    const uint32_t ko = __shfl_sync(0xffffffffu, k[f], l), io = __shfl_sync(0xffffffffu, id[f], l);
-#pragma unroll
-                    for (int e = 0; e < kWarpSortMax / 32; ++e) rank[e] += (ko < k[e] || (ko == k[e] && io < id[e])) ? 1u : 0u;
-                }
-            }
-        }
-#pragma unroll
-        for (int e = 0; e < kWarpSortMax / 32; ++e)
-            if (id[e] != 0xffffffffu) a.flatten_ids[gstart + rank[e]] = (int32_t)id[e];
-    }
-    // still larger groups (rare): re-emit the chunk's runs that cover the tile, in run (= depth) order
-    uint32_t big = __ballot_sync(0xffffffffu, c > (uint32_t)kWarpSortMax);
-    while (big) {
-        const int src = __ffs(big) - 1;
-        big &= big - 1;
-        const uint32_t gp = __shfl_sync(0xffffffffu, p, src), gt = __shfl_sync(0xffffffffu, t, src);
-        const uint32_t gstart = __shfl_sync(0xffffffffu, start, src), gc = __shfl_sync(0xffffffffu, c, src);
-        const uint32_t ra = a.chunk_run[gp], rb = a.chunk_run[gp + 1];
-        const uint32_t cam = gt / a.n_tiles, tl = gt - cam * a.n_tiles;
-        const uint32_t ty = tl / a.tile_width, tx = tl - ty * a.tile_width;
-        uint32_t written = 0;
-        for (uint32_t r0 = ra; r0 < rb && written < gc; r0 += 32) {
-            const uint32_t r = r0 + lane;
-            bool cover = false;
-            uint32_t idx = 0;
-            if (r < rb) {
-                idx = a.rt.idx[r];
-                const uint2 b = a.rt.box[r];
-                const uint32_t x0 = b.x & 0xffffu, y0 = b.x >> 16, w = b.y & 0xffffu, h = b.y >> 16;
-                cover = tx >= x0 && tx < x0 + w && ty >= y0 && ty < y0 + h && (!a.multi_cam || idx / a.N == cam);
-                if constexpr (kFilter) {
-                    if (cover)
-                        cover = (w * h <= 32u) ? ((a.rt.mask[r] >> ((ty - y0) * w + (tx - x0))) & 1u) != 0u
-                                               : ewa_tile_contributes(prim_filter(a.rt, idx), tx, ty);
-                }
-            }
-            const uint32_t m = __ballot_sync(0xffffffffu, cover);
-            const uint32_t pos = gstart + written + __popc(m & ((1u << lane) - 1u));
-            if (cover && pos < gstart + gc) a.flatten_ids[pos] = (int32_t)idx;
-            written += __popc(m);
-        }
-    }
-}
-
-template <bool kScatter, bool kFilter = false>
-__global__ void __launch_bounds__(kBinThreads) tile_bin_kernel(const BinArgs a) {
+template <bool kFilter = false>
+__global__ void __launch_bounds__(kBinThreads) tile_hist_kernel(const BinArgs a) {
     extern __shared__ uint32_t s_cnt[]; // [t_cnt]
     __shared__ uint32_t s_range[2];
-    __shared__ uint32_t s_nwork[2];
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     const uint32_t p = blockIdx.x;
-    if (tid < 2) s_nwork[tid] = 0;
     uint32_t *row = a.M + (size_t)p * a.T_total + a.t_lo;
     const unsigned long long I = a.ctl->n_isects;
     const uint32_t n_runs = a.ctl->n_runs;
     if (tid < 32) {
-        const uint32_t ra = kScatter ? a.chunk_run[p] : chunk_first_run(a, p, I, n_runs);
-        const uint32_t rb = kScatter ? a.chunk_run[p + 1] : chunk_first_run(a, p + 1, I, n_runs);
+        const uint32_t ra = chunk_first_run(a, p, I, n_runs);
+        const uint32_t rb = chunk_first_run(a, p + 1, I, n_runs);
         if (tid == 0) {
             s_range[0] = ra; s_range[1] = rb;
-            if (!kScatter) {
-                a.chunk_run[p] = ra;
-                if (p == a.P - 1) a.chunk_run[a.P] = n_runs;
-            }
+            a.chunk_run[p] = ra;
+            if (p == a.P - 1) a.chunk_run[a.P] = n_runs;
         }
     }
-    if (kScatter) {
-        for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) s_cnt[t] = row[t];
-    } else {
-        for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) s_cnt[t] = 0;
-    }
+    for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) s_cnt[t] = 0;
     __syncthreads();
     const uint32_t ra = s_range[0], rb = s_range[1];
 
-    auto place = [&](uint32_t idx, uint32_t cam_base, uint32_t x, uint32_t y) {
-        const uint32_t g = cam_base + y * a.tile_width + x - a.t_lo;
-        if (g < a.t_cnt) {
-            const uint32_t pos = atomicAdd(&s_cnt[g], 1u);
-            if (kScatter && pos < a.cap) a.flatten_ids[pos] = (int32_t)idx;
-        }
-    };
     for (uint32_t r0 = ra + (tid & ~31u); r0 < rb; r0 += kBinThreads) { // warp-uniform trip count
         const uint32_t r = r0 + lane;
         uint32_t idx = 0, bx = 0, by = 0, tmask = 0xffffffffu;
@@ -576,11 +391,10 @@ __global__ void __launch_bounds__(kBinThreads) tile_bin_kernel(const BinArgs a) 
         const uint32_t cam_base = a.multi_cam ? (idx / a.N) * a.n_tiles : 0u;
         // runs of up to 32 tiles: one lane each
         if (n > 0 && n <= 32) {
-            // four tiles per trip: the four shared-memory atomics are in flight together (their return value, the
-            // slot, is what the store waits for)
+            // four tiles per trip: the four shared-memory atomics are in flight together
             uint32_t x = x0, y = y0;
             for (uint32_t j = 0; j < n; j += 4) {
-                uint32_t g[4], pos[4];
+                uint32_t g[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     bool take = j + u < n;
@@ -589,12 +403,8 @@ __global__ void __launch_bounds__(kBinThreads) tile_bin_kernel(const BinArgs a) 
                     if (++x == x0 + w) { x = x0; ++y; }
                 }
 #pragma unroll
-                for (int u = 0; u < 4; ++u) pos[u] = (g[u] < a.t_cnt) ? atomicAdd(&s_cnt[g[u]], 1u) : 0xffffffffu;
-                if (kScatter) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        if (pos[u] < a.cap) a.flatten_ids[pos[u]] = (int32_t)idx;
-                }
+                for (int u = 0; u < 4; ++u)
+                    if (g[u] < a.t_cnt) atomicAdd(&s_cnt[g[u]], 1u);
             }
         }
         // larger runs: the whole warp strides over the box
@@ -612,47 +422,86 @@ __global__ void __launch_bounds__(kBinThreads) tile_bin_kernel(const BinArgs a) 
                 if constexpr (kFilter) {
                     if (!ewa_tile_contributes(bf, bx0 + dx, by0 + dy)) continue;
                 }
-                place(bidx, bcam, bx0 + dx, by0 + dy);
+                const uint32_t g = bcam + (by0 + dy) * a.tile_width + bx0 + dx - a.t_lo;
+                if (g < a.t_cnt) atomicAdd(&s_cnt[g], 1u);
             }
         }
     }
     __syncthreads();
-    if (!kScatter) {
-        for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) row[t] = s_cnt[t];
-    } else {
-        // the CTA's own groups, while their slots are still in L2: row[] holds the first slot, the counter the end.
-        // Most groups have one member.  The tiles whose group needs sorting are compacted into a work list so that
-        // every lane of the repair loops has a group (they are chains of dependent gathers) -- groups of up to four
-        // from the front of the list, larger ones from the back, so that a warp runs ONE of the sorting paths.
-        uint16_t *work = reinterpret_cast<uint16_t *>(s_cnt + a.t_cnt);
-        for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) {
-            const uint32_t start = row[t], end = min(s_cnt[t], a.cap);
-            if (end > start + 1) {
-                if (end - start <= 4) work[atomicAdd(&s_nwork[0], 1u)] = (uint16_t)t;
-                else work[a.t_cnt - 1 - atomicAdd(&s_nwork[1], 1u)] = (uint16_t)t;
-            }
+    for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) row[t] = s_cnt[t];
+}
+
+template <bool kFilter = false>
+__global__ void __launch_bounds__(kBinThreads) tile_place_kernel(const BinArgs a) {
+    extern __shared__ uint32_t s_cnt[]; // [t_cnt]: next slot of every tile of the window
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t p = blockIdx.x;
+    const uint32_t *row = a.M + (size_t)p * a.T_total + a.t_lo;
+    const uint32_t ra = a.chunk_run[p], rb = a.chunk_run[p + 1];
+    for (uint32_t t = tid; t < a.t_cnt; t += kBinThreads) s_cnt[t] = row[t];
+    __syncthreads();
+
+    for (uint32_t r0 = ra; r0 < rb; r0 += 32) { // every warp walks every run
+        const uint32_t r = r0 + lane;
+        uint32_t idx = 0, bx = 0, by = 0, tmask = 0xffffffffu;
+        if (r < rb) {
+            idx = a.rt.idx[r];
+            const uint2 b = a.rt.box[r];
+            bx = b.x; by = b.y;
+            if constexpr (kFilter) tmask = a.rt.mask[r];
         }
-        __syncthreads();
-        const uint32_t n_small = s_nwork[0], n_large = s_nwork[1];
-        for (uint32_t i0 = tid & ~31u; i0 < n_small; i0 += kBinThreads) { // warp-uniform trip count
-            const uint32_t i = i0 + lane;
-            uint32_t t = 0, start = 0, c = 0;
-            if (i < n_small) {
-                t = work[i];
-                start = row[t];
-                c = min(s_cnt[t], a.cap) - start;
-            }
-            repair_small(a, a.depths, start, c);
+        const uint32_t w = by & 0xffffu, h = by >> 16; // 0 for the lanes past the chunk
+        const uint32_t x0 = bx & 0xffffu, y0 = bx >> 16;
+        const uint32_t y1 = y0 + ((warp - y0) & (kBinWarps - 1)); // this warp's first row of the box
+        const uint32_t n = y1 < y0 + h ? ((y0 + h - 1 - y1) / kBinWarps + 1) * w : 0u;
+        const uint32_t cam = a.multi_cam ? idx / a.N : 0u;
+        // inclusive scan of n: the lane's intersections are [end - n, end) of the step's flat sequence
+        uint32_t end = n;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, end, o);
+            if (lane >= (uint32_t)o) end += t;
         }
-        for (uint32_t i0 = tid & ~31u; i0 < n_large; i0 += kBinThreads) {
-            const uint32_t i = i0 + lane;
-            uint32_t t = 0, start = 0, c = 0;
-            if (i < n_large) {
-                t = work[a.t_cnt - 1 - i];
-                start = row[t];
-                c = min(s_cnt[t], a.cap) - start;
+        const uint32_t first = end - n, total = __shfl_sync(0xffffffffu, end, 31);
+        for (uint32_t e0 = 0; e0 < total; e0 += 32) { // warp-uniform
+            const uint32_t e = e0 + lane;
+            // owner: the last lane whose first intersection is <= e (a lane without intersections in this warp's rows
+            // shares its `first` with the next lane, so the last such lane has intersections)
+            uint32_t src = 0;
+#pragma unroll
+            for (uint32_t s = 16; s; s >>= 1)
+                if (__shfl_sync(0xffffffffu, first, src + s) <= e) src += s;
+            const uint32_t j = e - __shfl_sync(0xffffffffu, first, src);
+            const uint32_t ridx = __shfl_sync(0xffffffffu, idx, src);
+            const uint32_t rx0 = __shfl_sync(0xffffffffu, x0, src), ry1 = __shfl_sync(0xffffffffu, y1, src);
+            const uint32_t rw = max(__shfl_sync(0xffffffffu, w, src), 1u), rcam = __shfl_sync(0xffffffffu, cam, src);
+            const uint32_t k = j / rw, dx = j - k * rw;
+            const uint32_t x = rx0 + dx, y = ry1 + k * kBinWarps;
+            bool take = e < total;
+            if constexpr (kFilter) {
+                const uint32_t rmask = __shfl_sync(0xffffffffu, tmask, src), ry0 = __shfl_sync(0xffffffffu, y0, src);
+                const uint32_t rh = __shfl_sync(0xffffffffu, h, src);
+                if (take)
+                    take = (rw * rh <= 32u) ? ((rmask >> ((y - ry0) * rw + dx)) & 1u) != 0u
+                                            : ewa_tile_contributes(prim_filter(a.rt, ridx), x, y);
             }
-            repair_groups<kFilter>(a, a.depths, p, a.t_lo + t, start, c);
+            const uint32_t g = take ? rcam * a.n_tiles + y * a.tile_width + x - a.t_lo : 0xffffffffu;
+            take = g < a.t_cnt;
+            // the lanes of a round are in run order: a tile's members are ranked by lane.  Most rounds have no tile
+            // twice, which the atomic tells: every lane read its tile's counter before any lane advanced it.
+            uint32_t slot = take ? s_cnt[g] : 0u;
+            __syncwarp();
+            const uint32_t got = take ? atomicAdd(&s_cnt[g], 1u) : slot;
+            if (__any_sync(0xffffffffu, got != slot)) {
+                uint32_t rank = 0;
+                for (uint32_t l = 0; l < 32; ++l) {
+                    const uint32_t gl = __shfl_sync(0xffffffffu, g, l);
+                    rank += (l < lane && gl == g) ? 1u : 0u;
+                }
+                slot += rank;
+            }
+            __syncwarp();
+            if (take && slot < a.cap) a.flatten_ids[slot] = (int32_t)ridx;
         }
     }
 }
@@ -819,12 +668,11 @@ static SegPlan seg_plan(uint64_t n) {
     return s;
 }
 
-constexpr uint32_t kMaxWindowTiles = 36 * 1024; // 144 KB of counters (+ 72 KB work list in the scatter pass) at most
+constexpr uint32_t kMaxWindowTiles = 36 * 1024; // 144 KB of counters at most
 
 struct BinPlan {
     uint32_t T_total, t_win, n_win, P, S, seg_len;
-    size_t smem;         // counters of the histogram pass
-    size_t smem_scatter; // counters + 16-bit work list of the scatter pass
+    size_t smem; // counters of the histogram and placement passes
 };
 static BinPlan bin_plan(uint32_t C, uint32_t N, uint32_t tile_width, uint32_t tile_height) {
     const DeviceShape &d = device_shape();
@@ -835,7 +683,6 @@ static BinPlan bin_plan(uint32_t C, uint32_t N, uint32_t tile_width, uint32_t ti
     b.n_win = (b.T_total + b.t_win - 1) / b.t_win;
     if (b.n_win == 0) b.n_win = 1;
     b.smem = (size_t)b.t_win * 4;
-    b.smem_scatter = (size_t)b.t_win * 6;
     uint32_t per_sm = (uint32_t)((size_t)d.smem_sm / (b.smem + 1024));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 8) per_sm = 8; // 8 x 256 threads fill an SM
@@ -1084,21 +931,21 @@ static int plan_impl(uint32_t C, uint32_t N, const PlanSource &src, const float 
         BinArgs a;
         a.rt = rt; a.ctl = ctl; a.N = N; a.n_tiles = tile_width * tile_height; a.tile_width = tile_width;
         a.multi_cam = C > 1 ? 1u : 0u;
-        a.T_total = bp.T_total; a.P = bp.P; a.M = M; a.flatten_ids = nullptr; a.cap = 0; a.depths = nullptr;
+        a.T_total = bp.T_total; a.P = bp.P; a.M = M; a.flatten_ids = nullptr; a.cap = 0;
         a.chunk_run = reinterpret_cast<uint32_t *>(base + w.chunk_run);
         if (bp.smem > 48 * 1024) {
-            GSB_CUDA_TRY(cudaFuncSetAttribute(tile_bin_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+            GSB_CUDA_TRY(cudaFuncSetAttribute(tile_hist_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               (int)bp.smem));
-            GSB_CUDA_TRY(cudaFuncSetAttribute(tile_bin_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+            GSB_CUDA_TRY(cudaFuncSetAttribute(tile_hist_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               (int)bp.smem));
         }
         for (uint32_t wnd = 0; wnd < bp.n_win; ++wnd) {
             a.t_lo = wnd * bp.t_win;
             a.t_cnt = min(bp.t_win, bp.T_total - a.t_lo);
             if (src.ewa())
-                tile_bin_kernel<false, true><<<bp.P, kBinThreads, bp.smem, s>>>(a);
+                tile_hist_kernel<true><<<bp.P, kBinThreads, bp.smem, s>>>(a);
             else
-                tile_bin_kernel<false, false><<<bp.P, kBinThreads, bp.smem, s>>>(a);
+                tile_hist_kernel<false><<<bp.P, kBinThreads, bp.smem, s>>>(a);
             GSB_LAUNCH_CHECK();
         }
     }
@@ -1139,12 +986,12 @@ static int emit_impl(uint32_t C, uint32_t N, bool filter, const float4 *filt0, c
     a.multi_cam = C > 1 ? 1u : 0u;
     a.chunk_run = reinterpret_cast<uint32_t *>(base + w.chunk_run);
     a.T_total = bp.T_total; a.P = bp.P; a.M = reinterpret_cast<uint32_t *>(base + w.M);
-    a.flatten_ids = flatten_ids; a.cap = (uint32_t)n_isects; a.depths = depths;
-    if (bp.smem_scatter > 48 * 1024) {
-        GSB_CUDA_TRY(cudaFuncSetAttribute(tile_bin_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)bp.smem_scatter));
-        GSB_CUDA_TRY(cudaFuncSetAttribute(tile_bin_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)bp.smem_scatter));
+    a.flatten_ids = flatten_ids; a.cap = (uint32_t)n_isects;
+    if (bp.smem > 48 * 1024) {
+        GSB_CUDA_TRY(cudaFuncSetAttribute(tile_place_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)bp.smem));
+        GSB_CUDA_TRY(cudaFuncSetAttribute(tile_place_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)bp.smem));
     }
     {
         ProfScope ps("isect_emit", s);
@@ -1152,13 +999,15 @@ static int emit_impl(uint32_t C, uint32_t N, bool filter, const float4 *filt0, c
             a.t_lo = wnd * bp.t_win;
             a.t_cnt = min(bp.t_win, bp.T_total - a.t_lo);
             if (filter)
-                tile_bin_kernel<true, true><<<bp.P, kBinThreads, bp.smem_scatter, s>>>(a);
+                tile_place_kernel<true><<<bp.P, kBinThreads, bp.smem, s>>>(a);
             else
-                tile_bin_kernel<true, false><<<bp.P, kBinThreads, bp.smem_scatter, s>>>(a);
+                tile_place_kernel<false><<<bp.P, kBinThreads, bp.smem, s>>>(a);
             GSB_LAUNCH_CHECK();
         }
     }
-    if (isect_ids) { // only the operator API wants the 64-bit keys back (intersect_offset consumes them)
+    // only the operator API wants the 64-bit keys back (intersect_offset consumes them).  Written here, in order, rather
+    // than by the placing lane: scattered 8-byte stores to an array larger than L2 cost more than this pass.
+    if (isect_ids) {
         const uint32_t grid = (bp.T_total + kKeyWarps - 1) / kKeyWarps;
         ProfScope psk("isect_keys", s);
         isect_keys_kernel<<<grid, kIsectThreads, 0, s>>>((uint32_t)n_isects, reinterpret_cast<const uint32_t *>(base + w.toff),

@@ -180,9 +180,9 @@ GSB_API int gsb_isect_sort(uint64_t n_isects, uint32_t C, uint32_t tile_width, u
 
 /* Planned sorted path for sort == true: same outputs as gsb_isect_emit + gsb_isect_sort, bit for bit,
  * without sorting any intersection.  The Gaussians are ordered by depth once (N elements, own radix
- * sort), the runs in that order are cut into chunks, a per-(chunk, tile) histogram is scanned, every
- * intersection is written DIRECTLY into the final range of its (chunk, tile) group and the groups
- * (1-2 entries on average) are put into depth order in place (csrc/gsb_intersect.cu).  It is arranged around the one host read-back the
+ * sort), the runs in that order are cut into chunks, a per-(chunk, tile) histogram is scanned, and every
+ * intersection is written DIRECTLY to its final position, each (chunk, tile) group being filled in depth
+ * order (csrc/gsb_intersect.cu).  It is arranged around the one host read-back the
  * operator API forces: everything that does not need the host to know n_isects runs in the PLAN.
  *   gsb_isect_plan          tiles_per_gauss [C*N]; *n_isects_out (device OR pinned host int64,
  *                           written asynchronously on `stream`); tile_offsets_out [C*th*tw] int32 or
