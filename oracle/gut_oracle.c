@@ -10,8 +10,10 @@
  * kernels compute (all file:line citations are relative to /root/reference):
  *
  *   K1 projection (UT)      gsplat/ProjectionUT3DGSFused.cu:47-202,
- *                           gsplat/Cameras.cuh:33-71,228-240,257-280,346-369,
+ *                           gsplat/Cameras.cuh:33-71,228-240,257-320,346-413,
  *                           416-471,1034-1150, gsplat/Utils.cuh:171-179
+ *   a2 rolling shutter      gsplat/Cameras.cuh:268-413 (pose interpolation, frame time,
+ *                           shutter-pose projection and pixel rays), all four directions
  *   K2/K3 SH fwd/bwd        gsplat/SphericalHarmonicsCUDA.cu:21-371,374-399,445-481
  *   K4-K6 tile intersect    gsplat/IntersectTile.cu:47-113,218-251,
  *                           gsplat/Intersect.cpp:41-121
@@ -277,13 +279,34 @@ static Pose pose_from_viewmat(const float *se3) {
     p.t = v3_make(se3[3], se3[7], se3[11]);
     return p;
 }
-/* Cameras.cuh:268-280 with q_end == q_start, t_end == t_start (global shutter,
- * viewmats1 == nullptr: Cameras.cuh:54-56) */
-static Pose interpolate_pose_global(Pose s, real tau) {
+/* Cameras.cuh:33-71: the end pose is the start pose when viewmats1 == nullptr (:54-56) */
+static void shutter_poses(const float *viewmats0, const float *viewmats1, uint32_t cid, Pose *start, Pose *end) {
+    *start = pose_from_viewmat(viewmats0 + cid * 16);
+    *end = viewmats1 ? pose_from_viewmat(viewmats1 + cid * 16) : *start;
+}
+
+/* Cameras.cuh:268-280: lerp of t, GLM slerp of q */
+static Pose interpolate_pose(Pose s, Pose e, real tau) {
     Pose r;
-    r.t = v3_add(v3_scale(s.t, (real)1 - tau), v3_scale(s.t, tau));
-    r.q = quat_slerp(s.q, s.q, tau);
+    r.t = v3_add(v3_scale(s.t, (real)1 - tau), v3_scale(e.t, tau));
+    r.q = quat_slerp(s.q, e.q, tau);
     return r;
+}
+
+/* gsplat/Common.h ShutterType */
+enum { ORC_ROLLING_TOP_TO_BOTTOM = 0, ORC_ROLLING_LEFT_TO_RIGHT = 1, ORC_ROLLING_BOTTOM_TO_TOP = 2,
+       ORC_ROLLING_RIGHT_TO_LEFT = 3, ORC_GLOBAL = 4 };
+
+/* Cameras.cuh:288-320: relative frame time of an image point (0 for a global shutter).  The resolution is
+ * unsigned there, so (resolution - 1) is the integer W - 1 / H - 1 converted to floating point. */
+static real shutter_relative_frame_time(int rs_type, real px, real py, uint32_t W, uint32_t H) {
+    switch (rs_type) {
+    case ORC_ROLLING_TOP_TO_BOTTOM: return R_FLOOR(py) / (real)(H - 1);
+    case ORC_ROLLING_LEFT_TO_RIGHT: return R_FLOOR(px) / (real)(W - 1);
+    case ORC_ROLLING_BOTTOM_TO_TOP: return ((real)H - R_CEIL(py)) / (real)(H - 1);
+    case ORC_ROLLING_RIGHT_TO_LEFT: return ((real)W - R_CEIL(px)) / (real)(W - 1);
+    default: return 0;
+    }
 }
 
 /* Utils.cuh:80-102 quat_to_rotmat (normalising; rsqrt) -> column-major */
@@ -308,7 +331,7 @@ static m3 quat_to_rotmat(const real q4[4]) {
 }
 
 /* ------------------------------------------------------------------ */
-/* K1: UT projection (perfect pinhole, global shutter)                 */
+/* K1: UT projection (global and rolling shutter)                      */
 /* ------------------------------------------------------------------ */
 
 /* Cameras.cuh:228-240 */
@@ -321,7 +344,7 @@ static int in_bounds_margin(real px, real py, uint32_t W, uint32_t H, real margi
     return valid;
 }
 
-/* ---- camera models (Cameras.cuh:416-1001), global shutter ------------------------------- */
+/* ---- camera models (Cameras.cuh:416-1001) ----------------------------------------------- */
 enum { CM_PERFECT_PINHOLE = 0, CM_OPENCV_PINHOLE = 1, CM_OPENCV_FISHEYE = 2 };
 typedef struct {
     int kind;
@@ -471,6 +494,32 @@ static int cam_project(const CamModel *m, v3 cam, real margin, real *ox, real *o
     return in_bounds_margin(*ox, *oy, m->W, m->H, margin) && (theta <= m->max_angle);
 }
 
+/* world_point_to_image_point_shutter_pose (Cameras.cuh:346-413).  Global shutter: the start-pose projection.
+ * Rolling: project with the start and the end pose; seed from the start point if it is valid, else from the end
+ * point; if neither is valid, return the end point as invalid; else ten rounds of "row / column time of the current
+ * point -> interpolated pose -> projection", whose result is valid whatever the last projection says. */
+static int project_shutter_pose(const CamModel *cm, int rs_type, Pose s, Pose e, v3 pt, real margin, real *ox,
+                                real *oy) {
+    real sx, sy;
+    const int valid_start = cam_project(cm, v3_add(quat_rotate(s.q, pt), s.t), margin, &sx, &sy);
+    if (rs_type == ORC_GLOBAL) { *ox = sx; *oy = sy; return valid_start; }
+    real ex, ey;
+    const int valid_end = cam_project(cm, v3_add(quat_rotate(e.q, pt), e.t), margin, &ex, &ey);
+    real px, py;
+    if (valid_start) { px = sx; py = sy; }
+    else if (valid_end) { px = ex; py = ey; }
+    else { *ox = ex; *oy = ey; return 0; }
+    for (int j = 0; j < 10; ++j) {
+        const real tau = shutter_relative_frame_time(rs_type, px, py, cm->W, cm->H);
+        const Pose p = interpolate_pose(s, e, tau);
+        real nx, ny;
+        cam_project(cm, v3_add(quat_rotate(p.q, pt), p.t), margin, &nx, &ny);
+        px = nx; py = ny;
+    }
+    *ox = px; *oy = py;
+    return 1;
+}
+
 /* image_point_to_camera_ray (Cameras.cuh:457-470, 698-754, 961-1000): unit camera-space ray */
 static int cam_unproject(const CamModel *m, real px, real py, v3 *ray) {
     const real u0 = (px - m->cx) / m->fx, v0 = (py - m->cy) / m->fy;
@@ -540,23 +589,27 @@ static int cam_unproject(const CamModel *m, real px, real py, v3 *ray) {
  * ProjectionUT3DGSFused.cu:17-203.  Outputs for culled Gaussians: radii = 0,
  * everything else UNTOUCHED (the reference leaves at::empty garbage there,
  * Projection.cpp:70-73) -- compare under the radii>0 mask.
+ * viewmats1 (nullable) is the end-of-frame pose and rs_type the ShutterType; the centre-of-shutter pose
+ * (tau = 0.5) gives the near / far cull and the depth (:73-80), every sigma point goes through
+ * project_shutter_pose.
  */
 ORC_API int orc_projection_ut(
     uint32_t C, uint32_t N,
     const float *means, const float *quats, const float *scales, const float *opacities /*nullable*/,
-    const float *viewmats0, const float *viewmats1 /*must be NULL*/, const float *Ks,
+    const float *viewmats0, const float *viewmats1 /*nullable*/, const float *Ks,
     uint32_t image_width, uint32_t image_height,
     float eps2d_f, float near_plane, float far_plane, float radius_clip,
-    int camera_model, OrcUTParams ut, int global_shutter,
+    int camera_model, OrcUTParams ut, int rs_type,
     const float *radial, int n_radial, const float *tangential, int n_tangential, const float *thin_prism,
     int n_thin_prism,
     int32_t *radii, float *means2d, float *depths, float *conics, float *compensations /*nullable*/) {
-    if ((camera_model != ORC_PINHOLE && camera_model != ORC_FISHEYE) || viewmats1 || !global_shutter)
-        return ORC_E_UNSUPPORTED; /* rolling shutter / ortho: not restated */
+    if ((camera_model != ORC_PINHOLE && camera_model != ORC_FISHEYE) || rs_type < 0 || rs_type > ORC_GLOBAL)
+        return ORC_E_UNSUPPORTED; /* ortho: not restated */
     const real eps2d = eps2d_f;
     for (uint32_t cid = 0; cid < C; ++cid) {
-        const Pose start = pose_from_viewmat(viewmats0 + cid * 16);
-        const Pose mid = interpolate_pose_global(start, (real)0.5);
+        Pose start, end;
+        shutter_poses(viewmats0, viewmats1, cid, &start, &end);
+        const Pose mid = interpolate_pose(start, end, (real)0.5);
         const CamModel cm = cam_model_make(camera_model, image_width, image_height, Ks + cid * 9,
                                            radial ? radial + cid * n_radial : NULL, n_radial,
                                            tangential ? tangential + cid * n_tangential : NULL, n_tangential,
@@ -602,9 +655,9 @@ ORC_API int orc_projection_ut(
             real mx = 0, my = 0;
             int early = 0;
             for (int i = 0; i < 7; ++i) {
-                v3 cam = v3_add(quat_rotate(start.q, pts[i]), start.t);
                 real px, py;
-                int pv = cam_project(&cm, cam, (real)ut.in_image_margin_factor, &px, &py);
+                int pv = project_shutter_pose(&cm, rs_type, start, end, pts[i], (real)ut.in_image_margin_factor, &px,
+                                              &py);
                 if (ut.require_all_sigma_points_valid) {
                     valid &= pv;
                     if (!pv) { early = 1; break; }
@@ -999,13 +1052,13 @@ ORC_API int orc_isect_offsets(int64_t n_isects, const int64_t *isect_ids, uint32
 
 typedef struct { v3 o, d; int valid; } Ray;
 
-/* Cameras.cuh:322-339,261-265 (global shutter: shutter_relative_frame_time == 0, :297-317) */
-static Ray pixel_ray(real px, real py, const CamModel *cm, Pose start) {
+/* Cameras.cuh:322-339,261-265: the pose of the frame time of (px, py) itself, the pixel centre */
+static Ray pixel_ray(real px, real py, const CamModel *cm, Pose start, Pose end, int rs_type) {
     v3 cam;
     Ray r;
     r.valid = cam_unproject(cm, px, py, &cam);
     if (!r.valid) { r.o = v3_make(0, 0, 0); r.d = v3_make(0, 0, 0); return r; }
-    Pose p = interpolate_pose_global(start, (real)0);
+    Pose p = interpolate_pose(start, end, shutter_relative_frame_time(rs_type, px, py, cm->W, cm->H));
     m3 R_inv = mat3_cast(quat_inverse(p.q));
     r.o = m3_mulv(&R_inv, v3_scale(p.t, (real)-1));
     r.d = m3_mulv(&R_inv, cam);
@@ -1046,6 +1099,7 @@ static m3 iscl_rot_of(const float *quat4, const float *scale3) {
  * RasterizeToPixelsFromWorld3DGSFwd.cu:20-279 (CDIM == 3, C == 1 per call is
  * what the reference supports: flatten_ids index means[] directly, :197-200).
  * masks: [C, th, tw] bytes or NULL; backgrounds [C,3] or NULL.
+ * viewmats1 (nullable): end-of-frame poses; rs_type: ShutterType (Fwd.cu:80-127).
  * Outputs for masked-out tiles: only render_colors written (:143-150).
  */
 ORC_API int orc_raster_fwd(
@@ -1053,17 +1107,19 @@ ORC_API int orc_raster_fwd(
     const float *means, const float *quats, const float *scales, const float *colors,
     const float *opacities, const float *backgrounds, const uint8_t *masks,
     uint32_t image_width, uint32_t image_height, uint32_t tile_size,
-    const float *viewmats0, const float *Ks, int camera_model,
+    const float *viewmats0, const float *viewmats1, const float *Ks, int camera_model, int rs_type,
     const float *radial, int n_radial, const float *tangential, int n_tangential, const float *thin_prism,
     int n_thin_prism,
     const int32_t *tile_offsets, const int32_t *flatten_ids,
     float *render_colors, float *render_alphas, int32_t *last_ids) {
     if (camera_model != ORC_PINHOLE && camera_model != ORC_FISHEYE) return ORC_E_UNSUPPORTED;
+    if (rs_type < 0 || rs_type > ORC_GLOBAL) return ORC_E_UNSUPPORTED;
     (void)N;
     const uint32_t tile_width = (image_width + tile_size - 1) / tile_size;
     const uint32_t tile_height = (image_height + tile_size - 1) / tile_size;
     for (uint32_t cid = 0; cid < C; ++cid) {
-        const Pose start = pose_from_viewmat(viewmats0 + cid * 16);
+        Pose start, end;
+        shutter_poses(viewmats0, viewmats1, cid, &start, &end);
         const CamModel cm = cam_model_make(camera_model, image_width, image_height, Ks + cid * 9,
                                            radial ? radial + cid * n_radial : NULL, n_radial,
                                            tangential ? tangential + cid * n_tangential : NULL, n_tangential,
@@ -1097,7 +1153,7 @@ ORC_API int orc_raster_fwd(
                             for (int k = 0; k < 3; ++k) rc[pix * 3 + k] = bg ? bg[k] : 0.0f;
                             continue;
                         }
-                        const Ray ray = pixel_ray((real)j + (real)0.5, (real)i + (real)0.5, &cm, start);
+                        const Ray ray = pixel_ray((real)j + (real)0.5, (real)i + (real)0.5, &cm, start, end, rs_type);
                         real T = 1;
                         uint32_t cur_idx = 0;
                         real pix_out[3] = {0, 0, 0};
@@ -1178,7 +1234,7 @@ ORC_API int orc_raster_bwd(
     const float *means, const float *quats, const float *scales, const float *colors,
     const float *opacities, const float *backgrounds, const uint8_t *masks,
     uint32_t image_width, uint32_t image_height, uint32_t tile_size,
-    const float *viewmats0, const float *Ks, int camera_model,
+    const float *viewmats0, const float *viewmats1, const float *Ks, int camera_model, int rs_type,
     const float *radial, int n_radial, const float *tangential, int n_tangential, const float *thin_prism,
     int n_thin_prism,
     const int32_t *tile_offsets, const int32_t *flatten_ids,
@@ -1186,12 +1242,14 @@ ORC_API int orc_raster_bwd(
     const float *v_render_colors, const float *v_render_alphas,
     double *v_means, double *v_quats, double *v_scales, double *v_colors, double *v_opacities) {
     if (camera_model != ORC_PINHOLE && camera_model != ORC_FISHEYE) return ORC_E_UNSUPPORTED;
+    if (rs_type < 0 || rs_type > ORC_GLOBAL) return ORC_E_UNSUPPORTED;
     (void)N;
     if (n_isects == 0) return ORC_OK;
     const uint32_t tile_width = (image_width + tile_size - 1) / tile_size;
     const uint32_t tile_height = (image_height + tile_size - 1) / tile_size;
     for (uint32_t cid = 0; cid < C; ++cid) {
-        const Pose start = pose_from_viewmat(viewmats0 + cid * 16);
+        Pose start, end;
+        shutter_poses(viewmats0, viewmats1, cid, &start, &end);
         const CamModel cm = cam_model_make(camera_model, image_width, image_height, Ks + cid * 9,
                                            radial ? radial + cid * n_radial : NULL, n_radial,
                                            tangential ? tangential + cid * n_tangential : NULL, n_tangential,
@@ -1216,7 +1274,7 @@ ORC_API int orc_raster_bwd(
                         const uint32_t i = ty * tile_size + iy, j = tx * tile_size + ix;
                         if (!(i < image_height && j < image_width)) continue;
                         const uint64_t pix = (uint64_t)i * image_width + j;
-                        const Ray ray = pixel_ray((real)j + (real)0.5, (real)i + (real)0.5, &cm, start);
+                        const Ray ray = pixel_ray((real)j + (real)0.5, (real)i + (real)0.5, &cm, start, end, rs_type);
                         if (!ray.valid) continue; /* Bwd.cu:151: such pixels are never valid */
                         const real T_final = (real)1 - (real)ra_[pix];
                         real T = T_final;

@@ -21,6 +21,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIBS: dict[str, C.CDLL] = {}
 
 PINHOLE, ORTHO, FISHEYE = 0, 1, 2
+# gsplat/Common.h ShutterType
+ROLLING_TOP_TO_BOTTOM, ROLLING_LEFT_TO_RIGHT, ROLLING_BOTTOM_TO_TOP, ROLLING_RIGHT_TO_LEFT, GLOBAL = 0, 1, 2, 3, 4
 
 
 class OrcUTParams(C.Structure):
@@ -120,12 +122,13 @@ def _dist(radial, tangential, thin_prism, Cn):
 def projection_ut(means, quats, scales, opacities, viewmats, Ks, width, height, eps2d=0.3,
                   near_plane=0.01, far_plane=1e10, radius_clip=0.0, calc_compensations=False,
                   camera_model=PINHOLE, ut: UTParams | None = None, precision="f32", radial=None, tangential=None,
-                  thin_prism=None):
+                  thin_prism=None, viewmats1=None, rs_type=GLOBAL):
     """gsplat::projection_ut_3dgs_fused (Ops.h:69-98). Returns radii, means2d, depths, conics,
-    compensations (or None). Rows with radii == 0 hold zeros here (garbage in the reference)."""
+    compensations (or None). Rows with radii == 0 hold zeros here (garbage in the reference).
+    viewmats1: end-of-frame poses of a rolling shutter of type rs_type (None: the start poses)."""
     means, quats, scales = _f32(means), _f32(quats), _f32(scales)
     opacities = _f32(opacities)
-    viewmats, Ks = _f32(viewmats), _f32(Ks)
+    viewmats, Ks, viewmats1 = _f32(viewmats), _f32(Ks), _f32(viewmats1)
     Cn, N = viewmats.shape[0], means.shape[0]
     radii = np.zeros((Cn, N, 2), np.int32)
     means2d = np.zeros((Cn, N, 2), np.float32)
@@ -136,9 +139,9 @@ def projection_ut(means, quats, scales, opacities, viewmats, Ks, width, height, 
     dist, _keep = _dist(radial, tangential, thin_prism, Cn)
     rc = lib(precision).orc_projection_ut(
         C.c_uint32(Cn), C.c_uint32(N), _ptr(means), _ptr(quats), _ptr(scales), _ptr(opacities),
-        _ptr(viewmats), None, _ptr(Ks), C.c_uint32(width), C.c_uint32(height),
+        _ptr(viewmats), _ptr(viewmats1), _ptr(Ks), C.c_uint32(width), C.c_uint32(height),
         C.c_float(eps2d), C.c_float(near_plane), C.c_float(far_plane), C.c_float(radius_clip),
-        C.c_int(camera_model), ut.c(), C.c_int(1), *dist,
+        C.c_int(camera_model), ut.c(), C.c_int(rs_type), *dist,
         _ptr(radii, C.c_int32), _ptr(means2d), _ptr(depths), _ptr(conics), _ptr(comp))
     _check(rc, "projection_ut")
     return radii, means2d, depths, conics, comp
@@ -203,13 +206,13 @@ def isect_offsets(isect_ids, Cn, tile_width, tile_height):
 
 def raster_fwd(means, quats, scales, colors, opacities, backgrounds, masks, width, height,
                tile_size, viewmats, Ks, tile_offsets, flatten_ids, camera_model=PINHOLE,
-               precision="f32", radial=None, tangential=None, thin_prism=None):
+               precision="f32", radial=None, tangential=None, thin_prism=None, viewmats1=None, rs_type=GLOBAL):
     """gsplat::rasterize_to_pixels_from_world_3dgs_fwd (Ops.h:100-129)."""
     means, quats, scales = _f32(means), _f32(quats), _f32(scales)
     colors, opacities = _f32(colors), _f32(opacities)
     bg = _f32(backgrounds) if backgrounds is not None and np.size(backgrounds) else None
     m = None if masks is None else np.ascontiguousarray(masks, dtype=np.uint8)
-    viewmats, Ks = _f32(viewmats), _f32(Ks)
+    viewmats, Ks, viewmats1 = _f32(viewmats), _f32(Ks), _f32(viewmats1)
     toff = np.ascontiguousarray(tile_offsets, dtype=np.int32)
     flat = np.ascontiguousarray(flatten_ids, dtype=np.int32)
     Cn, N = viewmats.shape[0], means.shape[0]
@@ -219,9 +222,9 @@ def raster_fwd(means, quats, scales, colors, opacities, backgrounds, masks, widt
     rc = lib(precision).orc_raster_fwd(
         C.c_uint32(Cn), C.c_uint32(N), C.c_int64(flat.shape[0]), _ptr(means), _ptr(quats),
         _ptr(scales), _ptr(colors), _ptr(opacities), _ptr(bg), _ptr(m, C.c_uint8),
-        C.c_uint32(width), C.c_uint32(height), C.c_uint32(tile_size), _ptr(viewmats), _ptr(Ks),
-        C.c_int(camera_model), *_dist(radial, tangential, thin_prism, Cn)[0], _ptr(toff, C.c_int32),
-        _ptr(flat, C.c_int32), _ptr(renders), _ptr(alphas), _ptr(last_ids, C.c_int32))
+        C.c_uint32(width), C.c_uint32(height), C.c_uint32(tile_size), _ptr(viewmats), _ptr(viewmats1),
+        _ptr(Ks), C.c_int(camera_model), C.c_int(rs_type), *_dist(radial, tangential, thin_prism, Cn)[0],
+        _ptr(toff, C.c_int32), _ptr(flat, C.c_int32), _ptr(renders), _ptr(alphas), _ptr(last_ids, C.c_int32))
     _check(rc, "raster_fwd")
     return renders, alphas, last_ids
 
@@ -229,13 +232,13 @@ def raster_fwd(means, quats, scales, colors, opacities, backgrounds, masks, widt
 def raster_bwd(means, quats, scales, colors, opacities, backgrounds, masks, width, height,
                tile_size, viewmats, Ks, tile_offsets, flatten_ids, render_alphas, last_ids,
                v_render_colors, v_render_alphas, camera_model=PINHOLE, precision="f32", radial=None, tangential=None,
-               thin_prism=None):
+               thin_prism=None, viewmats1=None, rs_type=GLOBAL):
     """gsplat::rasterize_to_pixels_from_world_3dgs_bwd (Ops.h:131-165); float64 gradients."""
     means, quats, scales = _f32(means), _f32(quats), _f32(scales)
     colors, opacities = _f32(colors), _f32(opacities)
     bg = _f32(backgrounds) if backgrounds is not None and np.size(backgrounds) else None
     m = None if masks is None else np.ascontiguousarray(masks, dtype=np.uint8)
-    viewmats, Ks = _f32(viewmats), _f32(Ks)
+    viewmats, Ks, viewmats1 = _f32(viewmats), _f32(Ks), _f32(viewmats1)
     toff = np.ascontiguousarray(tile_offsets, dtype=np.int32)
     flat = np.ascontiguousarray(flatten_ids, dtype=np.int32)
     ra, li = _f32(render_alphas), np.ascontiguousarray(last_ids, dtype=np.int32)
@@ -250,9 +253,9 @@ def raster_bwd(means, quats, scales, colors, opacities, backgrounds, masks, widt
     rc = lib(precision).orc_raster_bwd(
         C.c_uint32(Cn), C.c_uint32(N), C.c_int64(flat.shape[0]), _ptr(means), _ptr(quats),
         _ptr(scales), _ptr(colors), _ptr(opacities), _ptr(bg), _ptr(m, C.c_uint8),
-        C.c_uint32(width), C.c_uint32(height), C.c_uint32(tile_size), _ptr(viewmats), _ptr(Ks),
-        C.c_int(camera_model), *_dist(radial, tangential, thin_prism, Cn)[0], _ptr(toff, C.c_int32),
-        _ptr(flat, C.c_int32), _ptr(ra),
+        C.c_uint32(width), C.c_uint32(height), C.c_uint32(tile_size), _ptr(viewmats), _ptr(viewmats1),
+        _ptr(Ks), C.c_int(camera_model), C.c_int(rs_type), *_dist(radial, tangential, thin_prism, Cn)[0],
+        _ptr(toff, C.c_int32), _ptr(flat, C.c_int32), _ptr(ra),
         _ptr(li, C.c_int32), _ptr(vrc), _ptr(vra), _ptr(v_means, D), _ptr(v_quats, D),
         _ptr(v_scales, D), _ptr(v_colors, D), _ptr(v_opac, D))
     _check(rc, "raster_bwd")
@@ -291,9 +294,11 @@ def add_noise(raw_opacities, raw_scales, raw_quats, noise, means, current_lr, pr
 # ---------------------------------------------------------------------------------------------
 
 def render_pipeline(scene: dict, precision="f32", with_bwd=False, v_render_colors=None,
-                    v_render_alphas=None):
+                    v_render_alphas=None, viewmats1=None, rs_type=GLOBAL):
     """Run projection -> SH -> intersect -> blend (and optionally the backward chain through
-    blend bwd and SH bwd) on a scene dict made by tests/scenes.py. C == 1."""
+    blend bwd and SH bwd) on a scene dict made by tests/scenes.py. C == 1.  viewmats1 / rs_type: a rolling
+    shutter's end-of-frame pose and direction (the SH directions use the start pose's camera centre)."""
+    rs = dict(viewmats1=viewmats1, rs_type=rs_type)
     W, H, ts = scene["width"], scene["height"], scene.get("tile_size", 16)
     tw, th = (W + ts - 1) // ts, (H + ts - 1) // ts
     means, quats, scales, opac = scene["means"], scene["quats"], scene["scales"], scene["opacities"]
@@ -302,7 +307,7 @@ def render_pipeline(scene: dict, precision="f32", with_bwd=False, v_render_color
     out = {}
     radii, means2d, depths, conics, _ = projection_ut(
         means, quats, scales, opac, viewmats, Ks, W, H, eps2d=0.3, near_plane=0.01,
-        far_plane=1e4, radius_clip=0.0, precision=precision)
+        far_plane=1e4, radius_clip=0.0, precision=precision, **rs)
     out.update(radii=radii, means2d=means2d, depths=depths, conics=conics)
     campos = np.linalg.inv(viewmats.astype(np.float64))[:, :3, 3].astype(np.float32)  # rasterizer.cpp:250-251
     dirs = means[None, :, :] - campos[:, None, :]
@@ -316,14 +321,15 @@ def render_pipeline(scene: dict, precision="f32", with_bwd=False, v_render_color
     out.update(tiles_per_gauss=tpg, isect_ids=ids, flatten_ids=flat, tile_offsets=off)
     bg = scene.get("background")
     renders, alphas, last_ids = raster_fwd(means, quats, scales, colors_act, opac[None], bg, None, W, H,
-                                           ts, viewmats, Ks, off, flat, precision=precision)
+                                           ts, viewmats, Ks, off, flat, precision=precision, **rs)
     out.update(renders=renders, alphas=alphas, last_ids=last_ids)
     if with_bwd:
-        backward_pipeline(scene, out, v_render_colors, v_render_alphas, precision)
+        backward_pipeline(scene, out, v_render_colors, v_render_alphas, precision, **rs)
     return out
 
 
-def backward_pipeline(scene: dict, out: dict, v_render_colors, v_render_alphas, precision="f32"):
+def backward_pipeline(scene: dict, out: dict, v_render_colors, v_render_alphas, precision="f32", viewmats1=None,
+                      rs_type=GLOBAL):
     """Backward chain of render_pipeline's forward `out` (blend bwd -> clamp -> SH bwd); adds the
     gradients to `out` in place and returns it."""
     W, H, ts = scene["width"], scene["height"], scene.get("tile_size", 16)
@@ -331,7 +337,8 @@ def backward_pipeline(scene: dict, out: dict, v_render_colors, v_render_alphas, 
     sh, deg = scene["sh_coeffs"], scene["sh_degree"]
     g = raster_bwd(means, quats, scales, out["colors"], opac[None], scene.get("background"), None, W, H, ts,
                    scene["viewmats"], scene["Ks"], out["tile_offsets"], out["flatten_ids"], out["alphas"],
-                   out["last_ids"], v_render_colors, v_render_alphas, precision=precision)
+                   out["last_ids"], v_render_colors, v_render_alphas, precision=precision, viewmats1=viewmats1,
+                   rs_type=rs_type)
     out.update(v_means=g[0], v_quats=g[1], v_scales=g[2], v_colors=g[3], v_opacities=g[4])
     # clamp_min(+0.5) backward, then SH backward (rasterizer_autograd.cpp:84-132)
     v_sh_colors = (g[3] * ((out["sh_colors"] + 0.5) > 0)).astype(np.float32)

@@ -6,7 +6,8 @@ do not cover: UT projection and from-world blend forward / backward (SURVEY.md 8
 Where the reference library was not built (build() makes it where the reference's sources are present),
 the CPU oracle stands in for it: tests/test_oracle_vs_reference_golden.py pins the oracle to stored outputs of
 those kernels, and test_gpu_vs_reference_golden.py compares this library with the stored outputs directly.  The rolling-shutter tests
-need the reference's precise build (the oracle restates the global shutter only) and skip without it."""
+here need the reference's precise build and skip without it; test_gpu_rolling_shutter.py checks that mode against the
+float64 oracle and the stored outputs of the precise build everywhere."""
 import os
 
 import numpy as np
@@ -324,8 +325,8 @@ def test_distorted_cameras_reference_vs_b200(native, ref, cuda_device, model):
 
 
 # ------------------------------------------------------------------------------------------
-# a2: rolling shutter (Cameras.cuh:268-413) -- per-pixel camera poses; pinned by the reference's kernels only
-# (the CPU oracle restates the global shutter: "parity unpinned" on the CPU side for this mode)
+# a2: rolling shutter (Cameras.cuh:268-413) -- per-pixel camera poses; here against the reference's kernels (the float64
+# oracle and the stored reference outputs: test_gpu_rolling_shutter.py)
 # ------------------------------------------------------------------------------------------
 RS_IDS = ["top_to_bottom", "left_to_right", "bottom_to_top", "right_to_left"]
 

@@ -155,15 +155,26 @@ def test_blend_unprojection_inverts_the_projection(orc, cam):
     assert moved > 1.0  # the distortion is not a no-op: off-centre points land more than a pixel from the ideal pinhole
 
 
-@pytest.mark.parametrize("cam", [dict(camera_model=0), OPENCV, FISHEYE], ids=["pinhole", "opencv", "fisheye"])
-def test_backward_matches_finite_differences_without_cutoffs(orc, cam):
+# (camera, rolling-shutter direction or None for the global shutter); the ids of the global cases are the camera's
+FD_CASES = [(dict(camera_model=0), None), (OPENCV, None), (FISHEYE, None), (dict(camera_model=0), 0), (OPENCV, 1),
+            (FISHEYE, 2), (dict(camera_model=0), 3)]
+FD_IDS = ["pinhole", "opencv", "fisheye", "pinhole-rolling_top_to_bottom", "opencv-rolling_left_to_right",
+          "fisheye-rolling_bottom_to_top", "pinhole-rolling_right_to_left"]
+
+
+@pytest.mark.parametrize("cam,rs_type", FD_CASES, ids=FD_IDS)
+def test_backward_matches_finite_differences_without_cutoffs(orc, cam, rs_type):
     """The analytic backward against central differences of the forward, camera model by camera model, on the
     test-only ORC_SMOOTH float64 build of the oracle (no 1/255 cut, no T <= 1e-4 stop): with fixed intersection
     lists the forward is then smooth, so the comparison is tight (1 %) on EVERY checked component instead of
-    "some step size agrees up to a threshold crossing".  The cut-offs themselves only gate which pairs contribute."""
+    "some step size agrees up to a threshold crossing".  The cut-offs themselves only gate which pairs contribute.
+    The rolling-shutter cases give every pixel its own pose, between the start pose and one turned by 3 degrees."""
     sc = scenes.scene_small(N=300, width=80, height=64, sh_degree=0, view=2)
     W, H = sc["width"], sc["height"]
     tw, th = (W + 15) // 16, (H + 15) // 16
+    if rs_type is not None:
+        from test_oracle_rolling_shutter import end_pose
+        cam = dict(cam, viewmats1=end_pose(sc["viewmats"], deg=3.0), rs_type=rs_type)
     rng = np.random.default_rng(8)
     colors = rng.random((1, 300, 3), dtype=np.float32)
     vrc = rng.standard_normal((1, H, W, 3))
