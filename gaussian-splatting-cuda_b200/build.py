@@ -44,9 +44,11 @@ CUDA_SOURCES = [
     ("gsb_optim.cu", []),
     ("gsb_fastgs.cu", []),
     ("gsb_bilagrid.cu", []),
+    ("gsb_mcmc.cu", []),
 ]
-CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh"]
-SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
+CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh",
+                "gsb_relocation.cuh"]
+SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
 
 
 def _run(cmd: list[str], verbose: bool) -> str:

@@ -214,35 +214,43 @@ __device__ __forceinline__ T block_scan_inclusive(T v, T *s_warp /* [kSortWarps]
     return v + add;
 }
 
-// ---- int32 counts -> inclusive int64 scan (the unsorted path's cum_tiles; Intersect.cpp:71) --------------
-__global__ void __launch_bounds__(kSortThreads) scan_blocksum_kernel(const int32_t *__restrict__ counts, uint64_t n,
-                                                                     uint32_t seg, long long *__restrict__ bsum) {
-    __shared__ long long s_warp[kSortWarps];
+// ---- inclusive scan of loader values: Load is `Acc operator()(uint64_t i) const` ---------------------------
+// Instantiated for int32 counts -> int64 (the unsorted path's cum_tiles; Intersect.cpp:71) and, in gsb_mcmc.cu, for
+// 0/1 flags -> int32 ranks and float weights -> a float64 prefix.
+struct LoadI32 {
+    const int32_t *p;
+    __device__ __forceinline__ long long operator()(uint64_t i) const { return p[i]; }
+};
+
+template <typename Load, typename Acc>
+__global__ void __launch_bounds__(kSortThreads) scan_blocksum_kernel(const Load load, uint64_t n, uint32_t seg,
+                                                                     Acc *__restrict__ bsum) {
+    __shared__ Acc s_warp[kSortWarps];
     const SegRange r = cta_segment(n, seg);
-    long long acc = 0;
-    for (uint64_t i = r.lo + threadIdx.x; i < r.hi; i += kSortThreads) acc += counts[i];
-    long long tot;
-    block_scan_inclusive<long long>(acc, s_warp, tot);
+    Acc acc = 0;
+    for (uint64_t i = r.lo + threadIdx.x; i < r.hi; i += kSortThreads) acc += load(i);
+    Acc tot;
+    block_scan_inclusive<Acc>(acc, s_warp, tot);
     if (threadIdx.x == 0) bsum[blockIdx.x] = tot;
 }
 
-__global__ void __launch_bounds__(kSortThreads) scan_apply_kernel(const int32_t *__restrict__ counts, uint64_t n,
-                                                                  uint32_t seg, const long long *__restrict__ bsum,
-                                                                  int64_t *__restrict__ cum) {
-    __shared__ long long s_warp[kSortWarps];
-    long long carry;
+template <typename Load, typename Acc, typename Out>
+__global__ void __launch_bounds__(kSortThreads) scan_apply_kernel(const Load load, uint64_t n, uint32_t seg,
+                                                                  const Acc *__restrict__ bsum, Out *__restrict__ cum) {
+    __shared__ Acc s_warp[kSortWarps];
+    Acc carry;
     {
-        long long part = 0;
+        Acc part = 0;
         for (uint32_t bb = threadIdx.x; bb < blockIdx.x; bb += kSortThreads) part += bsum[bb];
-        block_scan_inclusive<long long>(part, s_warp, carry);
+        block_scan_inclusive<Acc>(part, s_warp, carry);
     }
     const SegRange r = cta_segment(n, seg);
     for (uint64_t i0 = r.lo; i0 < r.hi; i0 += kSortThreads) {
         const uint64_t i = i0 + threadIdx.x;
-        const long long v = i < r.hi ? (long long)counts[i] : 0;
-        long long tot;
-        const long long inc = block_scan_inclusive<long long>(v, s_warp, tot);
-        if (i < r.hi) cum[i] = (int64_t)(carry + inc);
+        const Acc v = i < r.hi ? load(i) : (Acc)0;
+        Acc tot;
+        const Acc inc = block_scan_inclusive<Acc>(v, s_warp, tot);
+        if (i < r.hi) cum[i] = (Out)(carry + inc);
         carry += tot;
     }
 }

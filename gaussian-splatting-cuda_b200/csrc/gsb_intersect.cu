@@ -779,9 +779,9 @@ extern "C" int gsb_isect_count(uint32_t C, uint32_t N, const float *means2d, con
     GSB_LAUNCH_CHECK();
     const SegPlan sp = seg_plan(n);
     long long *bsum = reinterpret_cast<long long *>(workspace);
-    scan_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(tiles_per_gauss, n, sp.seg, bsum);
+    scan_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{tiles_per_gauss}, n, sp.seg, bsum);
     GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(tiles_per_gauss, n, sp.seg, bsum, cum_tiles);
+    scan_apply_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{tiles_per_gauss}, n, sp.seg, bsum, cum_tiles);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }

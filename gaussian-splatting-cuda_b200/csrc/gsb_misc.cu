@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "gsb_common.cuh"
+#include "gsb_relocation.cuh"
 
 namespace gsb {
 
@@ -63,11 +64,7 @@ __global__ void __launch_bounds__(kMiscThreads) quat_to_rotmat_kernel(uint32_t N
         for (int c = 0; c < 3; ++c) o[r * 3 + c] = R.m[r][c];
 }
 
-// gsplat::relocation (RelocationCUDA.cu:12-43): Eq. (9) of "3D Gaussian Splatting as Markov Chain Monte Carlo".
-// A Gaussian split into n copies keeps its appearance with opacity o' = 1 - (1 - o)^(1/n) and scales multiplied by
-//     o / sum_{i=1..n} sum_{k=0..i-1} C(i-1, k) (-1)^k o'^(k+1) / sqrt(k+1).
-// The double sum is evaluated k-major here: the power of o' and 1/sqrt(k+1) are built once per k (no powf in the
-// loop) and multiplied by the column sum of the caller's binomial table, sum_{i=k+1..n} binoms[i-1][k].
+// gsplat::relocation (RelocationCUDA.cu:12-43); the body is relocation_one (gsb_relocation.cuh).
 __global__ void __launch_bounds__(kMiscThreads) relocation_kernel(uint32_t N, const float *__restrict__ opacities,
                                                                    const float *__restrict__ scales,
                                                                    const int32_t *__restrict__ ratios,
@@ -76,31 +73,24 @@ __global__ void __launch_bounds__(kMiscThreads) relocation_kernel(uint32_t N, co
                                                                    float *__restrict__ new_scales) {
     const uint32_t g = blockIdx.x * kMiscThreads + threadIdx.x;
     if (g >= N) return;
-    const int copies = ratios[g];
-    const float o = opacities[g];
-    const float o_new = 1.0f - powf(1.0f - o, 1.0f / (float)copies);
-    new_opacities[g] = o_new;
-    float series = 0.0f;
-    float pw = o_new; // (-1)^k o'^(k+1), k = 0
-    for (int k = 0; k < copies; ++k) {
-        float column = 0.0f;
-        for (int i = k + 1; i <= copies; ++i) column += binoms[(i - 1) * n_max + k];
-        series += column * pw * rsqrtf((float)(k + 1));
-        pw *= -o_new;
-    }
-    const float grow = o / series;
+    const float grow = relocation_one(opacities[g], ratios[g], binoms, n_max, &new_opacities[g]);
     new_scales[(size_t)g * 3] = grow * scales[(size_t)g * 3];
     new_scales[(size_t)g * 3 + 1] = grow * scales[(size_t)g * 3 + 1];
     new_scales[(size_t)g * 3 + 2] = grow * scales[(size_t)g * 3 + 2];
 }
 
+// kLrOnDevice: the rate is *lr_dev * lr_scale, read at run time (gsb_mcmc_add_noise), so a captured CUDA graph
+// follows the learning-rate schedule; otherwise it is the launch argument current_lr (gsb_add_noise).
+template <bool kLrOnDevice>
 __global__ void __launch_bounds__(kMiscThreads) add_noise_kernel(uint32_t N, const float *__restrict__ raw_opacities,
                                                                   const float *__restrict__ raw_scales,
                                                                   const float *__restrict__ raw_quats,
                                                                   const float *__restrict__ noise,
-                                                                  float *__restrict__ means, float current_lr) {
+                                                                  float *__restrict__ means, float current_lr,
+                                                                  const float *__restrict__ lr_dev, float lr_scale) {
     const uint32_t idx = blockIdx.x * kMiscThreads + threadIdx.x;
     if (idx >= N) return;
+    if (kLrOnDevice) current_lr = __ldg(lr_dev) * lr_scale; // mcmc.cpp:353: (float)lr * _noise_lr
     const size_t i3 = (size_t)idx * 3;
     const float e0 = expf(2.f * raw_scales[i3]), e1 = expf(2.f * raw_scales[i3 + 1]), e2 = expf(2.f * raw_scales[i3 + 2]);
     const float4 q = reinterpret_cast<const float4 *>(raw_quats)[idx];
@@ -145,8 +135,22 @@ extern "C" int gsb_add_noise(uint32_t N, const float *raw_opacities, const float
                              const float *noise, float *means, float current_lr, gsb_stream_t stream) {
     if (N == 0) return GSB_OK;
     if (!raw_opacities || !raw_scales || !raw_quats || !noise || !means) return GSB_E_INVALID;
-    gsb::add_noise_kernel<<<(N + gsb::kMiscThreads - 1) / gsb::kMiscThreads, gsb::kMiscThreads, 0,
-                            gsb::as_stream(stream)>>>(N, raw_opacities, raw_scales, raw_quats, noise, means, current_lr);
+    gsb::add_noise_kernel<false><<<(N + gsb::kMiscThreads - 1) / gsb::kMiscThreads, gsb::kMiscThreads, 0,
+                                   gsb::as_stream(stream)>>>(N, raw_opacities, raw_scales, raw_quats, noise, means,
+                                                             current_lr, nullptr, 0.f);
+    GSB_LAUNCH_CHECK();
+    return GSB_OK;
+}
+
+extern "C" int gsb_mcmc_add_noise(uint32_t N, const float *raw_opacities, const float *raw_scales,
+                                  const float *raw_quats, const float *noise, float *means, const float *lr,
+                                  float lr_scale, gsb_stream_t stream) {
+    if (N == 0) return GSB_OK;
+    if (!raw_opacities || !raw_scales || !raw_quats || !noise || !means || !lr) return GSB_E_INVALID;
+    if (reinterpret_cast<uintptr_t>(raw_quats) & 15) return GSB_E_INVALID;
+    gsb::add_noise_kernel<true><<<(N + gsb::kMiscThreads - 1) / gsb::kMiscThreads, gsb::kMiscThreads, 0,
+                                  gsb::as_stream(stream)>>>(N, raw_opacities, raw_scales, raw_quats, noise, means,
+                                                            0.f, lr, lr_scale);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }

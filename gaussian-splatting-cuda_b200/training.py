@@ -6,6 +6,9 @@
                      iterations), all groups stepped by ONE kernel launch (gsb_adam_step)
   TrainStep          render (extended operator on the raw tensors) -> loss -> backward -> Adam [-> MCMC noise], with
                      the intersection buffer sized from a capacity so that the iteration has no host read-back
+  strategy           optional MCMC densification (SURVEY.md 8 f6, mcmc.py): render -> loss -> backward -> regularisers
+                     -> post_backward (SH bump, relocation / growth on refine iterations, noise) -> Adam (nothing to
+                     step on a growth iteration) -> scheduler
   bilateral_grid     optional (SURVEY.md 8 f5, trainer.cpp:662-665,698-705,758-762): render -> slice through the
                      image's grid -> unclamped loss -> + weight * TV of all grids -> backward -> one Adam launch for the
                      Gaussians and the grids (lr from the warm-up/exponential schedule, eps 1e-15)
@@ -13,6 +16,7 @@
 Everything that computes lives behind the C ABI; this file only orders the calls, like the reference's trainer does."""
 from __future__ import annotations
 
+import dataclasses
 import math
 from dataclasses import dataclass, field
 
@@ -20,6 +24,7 @@ import torch
 
 from . import _product_ns, load, rasterize_fused
 from .bilateral import BilateralGrid, WarmupExponentialLR
+from .mcmc import MCMC, growth_count
 
 
 class _PhotometricLoss(torch.autograd.Function):
@@ -211,6 +216,10 @@ class TrainStep:
     bilateral_grid_lr: float = 2e-3
     tv_loss_weight: float = 10.0                 # mcmc_optimization_params.json (default_optimization_params.json: 5)
     grid_state: _GridState | None = None         # created on first use
+    strategy: MCMC | None = None                 # MCMC densification: owns params and the optimizer's moments
+
+    def __post_init__(self):
+        _check_strategy(self.strategy, self.mcmc_noise_lr, self.params, self.optimizer, self.sh_degree)
 
     def _grid(self) -> _GridState:
         if self.grid_state is None:
@@ -221,6 +230,8 @@ class TrainStep:
     def __call__(self, viewmat, K, target, background=None, image_idx=None):
         P = self.params
         self.iteration += 1
+        if self.strategy is not None:
+            self.sh_degree = self.strategy.sh_degree
         out = rasterize_fused(P["means"], P["sh0"], P["shN"], P["scaling_raw"], P["rotation_raw"], P["opacity_raw"],
                               self.sh_degree, viewmat, K, self.width, self.height, bg_color=background,
                               isect_capacity=self.capacity)
@@ -237,6 +248,7 @@ class TrainStep:
             loss.backward()
             G.grid.grids.grad = v_grids
             loss = loss.detach() + G.weight[0] * tv  # the trainer's loss_value includes the TV term
+        reg = _strategy_post_backward(self.strategy, self.iteration)
         if self.optimizer is not None:
             if self.bilateral_grid is not None:
                 extra = self.grid_state.adam_group()
@@ -250,7 +262,7 @@ class TrainStep:
             self.optimizer.zero_grad()
         if self.bilateral_grid is not None:
             self.bilateral_grid.grids.grad = None
-        self.last = {"n_isects": out.n_isects, "stats": stats}
+        self.last = {"n_isects": out.n_isects, "stats": stats, "reg": reg}
         return loss
 
     def size_capacity(self, viewmat, K, target, background=None, slack: float = 1.25):
@@ -262,6 +274,34 @@ class TrainStep:
             n = int(out.n_isects.item())
         self.capacity = int(n * slack) + 1024
         return n
+
+
+def _check_strategy(strategy, mcmc_noise_lr: float, params=None, optimizer=None, sh_degree=None) -> None:
+    """A strategy owns the parameter dict and the optimizer's moments: the step must use the same objects, and the
+    degree it renders with is the strategy's active degree (SplatData's, which the strategy raises)."""
+    if strategy is None:
+        return
+    if mcmc_noise_lr > 0.0:
+        raise ValueError("mcmc_noise_lr and strategy both add noise: the strategy injects it before Adam, as the "
+                         "reference does, so pass one of them")
+    if params is not None and params is not strategy.params:
+        raise ValueError("the step's params must be the strategy's params dict (growth replaces its tensors)")
+    if optimizer is not None and optimizer is not strategy.optimizer:
+        raise ValueError("the step's optimizer must be the strategy's optimizer (growth replaces its moments)")
+    if sh_degree is not None and int(sh_degree) != strategy.sh_degree:
+        raise ValueError(f"sh_degree {sh_degree} differs from the strategy's active degree {strategy.sh_degree}: "
+                         "pass MCMC(..., sh_degree=...) or the step the same degree")
+
+
+def _strategy_post_backward(strategy, iteration: int):
+    """Regularisers into the gradients, then the strategy's post_backward (trainer.cpp:668-756): on a growth iteration
+    the parameters become new leaves without gradients, so the following Adam step skips them."""
+    if strategy is None:
+        return None
+    with torch.no_grad():
+        reg = strategy.regularize()
+        strategy.post_backward(iteration)
+    return reg
 
 
 class GraphedTrainStep:
@@ -277,11 +317,16 @@ class GraphedTrainStep:
 
     def __init__(self, params: dict, sh_degree: int, width: int, height: int, cfg: AdamConfig | None = None,
                  lambda_dssim: float = 0.2, capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None,
-                 bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0):
+                 bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0, strategy: MCMC | None = None):
         load()
+        _check_strategy(strategy, 0.0, params, None, sh_degree)
         self.params, self.sh_degree, self.W, self.H = params, int(sh_degree), int(width), int(height)
         self.lambda_dssim = float(lambda_dssim)
-        self.opt = FusedAdam(params, cfg)
+        # with a strategy, its optimizer (whose moments live in the strategy's storage) is the step's
+        self.opt = strategy.optimizer if strategy is not None else FusedAdam(params, cfg)
+        self.strategy = strategy
+        self.graph_b = None
+        self.captures = 0
         self.slack = capacity_slack
         dev = params["means"].device
         self.dev = dev
@@ -302,7 +347,8 @@ class GraphedTrainStep:
         self.capacity = 0
         self.iteration = 0
 
-    def _body(self):
+    def _part_a(self):
+        """render -> loss -> backward [-> the strategy's regularisers]: (loss, stats, count, grid gradient or None)"""
         P, S = self.params, self.static
         out = rasterize_fused(P["means"], P["sh0"], P["shN"], P["scaling_raw"], P["rotation_raw"], P["opacity_raw"],
                               self.sh_degree, S["viewmat"], S["K"], self.W, self.H, bg_color=S["background"],
@@ -310,15 +356,84 @@ class GraphedTrainStep:
         if self.grid_state is None:
             loss, stats = photometric_loss(out.render_colors, S["target"], self.lambda_dssim)
             loss.backward()
-            self._adam()
-            return loss, stats, out.n_isects
+            self._regularize()
+            return loss, stats, out.n_isects, None
         G = self.grid_state
         tv, v_grids = G.tv()
         sliced = _SliceIntoGrad.apply(out.render_colors, G.grid.grids.detach(), G.idx, v_grids, False)
         loss, stats = photometric_loss_unclamped(sliced, S["target"], self.lambda_dssim)
         loss.backward()
+        self._regularize()
+        return loss.detach() + G.weight[0] * tv, stats, out.n_isects, v_grids
+
+    def _regularize(self):
+        if self.strategy is not None:
+            with torch.no_grad():
+                self.strategy.regularize()
+
+    def _part_b(self, v_grids):
+        """[the strategy's noise at the means group's rate, read from `dyn` ->] Adam"""
+        if self.strategy is not None:
+            self.strategy.inject_noise(self.dyn[0, 0:1])
         self._adam(v_grids)
-        return loss.detach() + G.weight[0] * tv, stats, out.n_isects
+
+    def _body(self):
+        loss, stats, n, v_grids = self._part_a()
+        self._part_b(v_grids)
+        return loss, stats, n
+
+    def _warm_up_and_capture(self):
+        """Warm-up iterations with every Adam group disabled and a zero noise rate (`dyn` is zero: nothing moves),
+        then the capture.  Without a strategy the iteration is one graph.  With one it is two graphs -- (render, loss,
+        backward, regularisers) and (noise, Adam) -- so that a refine can run eagerly between them, and the warm-up's
+        random draws are undone so that the replays draw what an eager run would."""
+        self.dyn.zero_()
+        rng = torch.cuda.get_rng_state(self.dev) if self.strategy is not None else None
+        side = torch.cuda.Stream(self.dev)
+        side.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(side):
+            for _ in range(3):
+                for p in self.params.values():
+                    p.grad = None
+                self._body()
+        torch.cuda.current_stream(self.dev).wait_stream(side)
+        for p in self.params.values():
+            p.grad = None
+        if rng is not None:
+            torch.cuda.set_rng_state(rng, self.dev)
+        self.graph = torch.cuda.CUDAGraph()
+        self.captures += 1
+        if self.strategy is None:
+            with torch.cuda.graph(self.graph):
+                self.loss, self.stats, self.n_isects = self._body()
+            return
+        with torch.cuda.graph(self.graph):
+            self.loss, self.stats, self.n_isects, v_grids = self._part_a()
+        self.graph_b = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph_b, pool=self.graph.pool()):
+            self._part_b(v_grids)
+
+    def _replay(self):
+        """One iteration from the captured graph(s).  With a strategy: part A, then -- on a refine iteration -- the
+        refine eagerly, then part B (noise, Adam).  A growth step replaces the parameters, so its noise runs eagerly on
+        the new rows, Adam has nothing to step (as FusedAdam after the reference's torch::cat) and the next call
+        re-captures; an SH-degree bump re-captures too.  A relocation-only refine works in place: no re-capture."""
+        st = self.strategy
+        if st is None:
+            self.graph.replay()
+            return
+        lr0 = self.opt.lr[0]  # the rate before this iteration's scheduler step
+        grows = st.is_refining(self.iteration) and growth_count(st.n, st.capacity) > 0
+        self._set_scalars(skip_adam=grows)
+        degree = st.sh_degree
+        self.graph.replay()
+        grew = st.refine(self.iteration)
+        if grew:
+            st.inject_noise(lr0)
+        else:
+            self.graph_b.replay()
+        if grew or st.sh_degree != degree:
+            self.graph = None
 
     def _adam(self, v_grids=None):
         """One launch for the Gaussians' groups (and the grids' after them), scalars from `dyn`."""
@@ -358,11 +473,12 @@ class GraphedTrainStep:
         if background is not None:
             S["background"].copy_(background.reshape(1, 3), non_blocking=True)
 
-    def _set_scalars(self):
-        """fused_adam.cpp:61-81 on the host: step counts, bias corrections, the shN freeze; strategy_utils.cpp:52-55 lr."""
+    def _set_scalars(self, skip_adam: bool = False):
+        """fused_adam.cpp:61-81 on the host: step counts, bias corrections, the shN freeze; strategy_utils.cpp:52-55 lr.
+        skip_adam: an iteration whose Adam step is skipped keeps the step counts (the learning rate still decays)."""
         o = self.opt
         for i, k in enumerate(PARAM_GROUPS):
-            o.steps[k] += 1
+            o.steps[k] += 0 if skip_adam else 1
             t = o.steps[k]
             enabled = 0.0 if (k == "shN" and self.iteration <= 1000) else 1.0
             self.dyn_host[i, 0] = o.lr[i]
@@ -382,6 +498,8 @@ class GraphedTrainStep:
 
     def capture(self, viewmat, K, target, background=None, image_idx=None):
         """Sizes the intersection capacity with one exact render, warms up and captures the graph."""
+        if self.strategy is not None:
+            self.sh_degree = self.strategy.sh_degree
         self._set_inputs(viewmat, K, target, background)
         if self.grid_state is not None:
             self.grid_state.set_image(image_idx)
@@ -391,20 +509,7 @@ class GraphedTrainStep:
                                   self.sh_degree, S["viewmat"], S["K"], self.W, self.H, bg_color=S["background"])
             n = int(out.n_isects.item())
         self.capacity = int(n * self.slack) + 1024
-        self.dyn.zero_()  # warm-up iterations must not move the parameters: every group disabled
-        side = torch.cuda.Stream(self.dev)
-        side.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(side):
-            for _ in range(3):
-                for p in self.params.values():
-                    p.grad = None
-                self._body()
-        torch.cuda.current_stream(self.dev).wait_stream(side)
-        for p in self.params.values():
-            p.grad = None
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.loss, self.stats, self.n_isects = self._body()
+        self._warm_up_and_capture()
         return n
 
     def __call__(self, viewmat, K, target, background=None, image_idx=None):
@@ -414,8 +519,9 @@ class GraphedTrainStep:
         self._set_inputs(viewmat, K, target, background)
         if self.grid_state is not None:
             self.grid_state.set_image(image_idx)
-        self._set_scalars()
-        self.graph.replay()
+        if self.strategy is None:
+            self._set_scalars()
+        self._replay()
         return self.loss
 
     def overflowed(self) -> bool:
@@ -445,6 +551,10 @@ class FastGsTrainStep:
     tv_loss_weight: float = 10.0
     grid_state: _GridState | None = None         # created on first use
     index_on_device: bool = False                # the graphed wrapper refreshes grid_state.idx itself before each replay
+    strategy: MCMC | None = None                 # MCMC densification: owns params and the optimizer's moments
+
+    def __post_init__(self):
+        _check_strategy(self.strategy, 0.0, self.params, self.optimizer, self.sh_degree)
 
     def _grid(self) -> _GridState:
         if self.grid_state is None:
@@ -469,6 +579,9 @@ class FastGsTrainStep:
         be = self.backend or fg.default_backend()
         P = self.params
         self.iteration += 1
+        if self.strategy is not None:
+            self.sh_degree = self.strategy.sh_degree
+            settings = dataclasses.replace(settings, active_sh_bases=(self.sh_degree + 1) ** 2)
         G = None
         if self.bilateral_grid is not None:
             G = self._grid()
@@ -498,13 +611,14 @@ class FastGsTrainStep:
                             P["shN"], w2c, settings, densification_info)
             for k, gk in zip(("means", "scaling_raw", "rotation_raw", "opacity_raw", "sh0", "shN"), g[:6]):
                 P[k].grad = gk.reshape(P[k].shape)
+        reg = _strategy_post_backward(self.strategy, self.iteration)
         if self.optimizer is not None:
             self.optimizer.step(self.iteration, G.adam_group() if G is not None else None)
             self.optimizer.zero_grad()
             if G is not None:
                 G.grid.grids.grad = None
         # capacity mode: the count is a device tensor (compare it with the capacity when convenient)
-        self.last = {"n_instances": ctx.get("n_instances_dev", int(ctx["ints"][1])), "stats": stats}
+        self.last = {"n_instances": ctx.get("n_instances_dev", int(ctx["ints"][1])), "stats": stats, "reg": reg}
         return stats[0] if G is None else stats[0] + G.weight[0] * tv
 
 
@@ -516,9 +630,9 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
 
     def __init__(self, params: dict, sh_degree: int, settings, cfg: AdamConfig | None = None, lambda_dssim: float = 0.2,
                  capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None, bilateral_grid_lr: float = 2e-3,
-                 tv_loss_weight: float = 10.0):
+                 tv_loss_weight: float = 10.0, strategy: MCMC | None = None):
         super().__init__(params, sh_degree, settings.width, settings.height, cfg, lambda_dssim, capacity_slack,
-                         bilateral_grid, bilateral_grid_lr, tv_loss_weight)
+                         bilateral_grid, bilateral_grid_lr, tv_loss_weight, strategy)
         from . import fastgs as fg
         dev = self.dev
         self.static = {"w2c": torch.zeros((4, 4), device=dev), "campos": torch.zeros((3,), device=dev),
@@ -532,12 +646,13 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
                                     backend=self.be, bilateral_grid=bilateral_grid, grid_state=self.grid_state,
                                     index_on_device=True)
 
-    def _body(self):
-        P, S = self.params, self.static
+    def _part_a(self):
+        S = self.static
         self.step.capacity = self.capacity
         loss = self.step(S["w2c"], self.settings, S["target"], S["background"])
-        self._adam(self.grid_state.grid.grids.grad if self.grid_state is not None else None)
-        return loss, self.step.last["stats"], self.step.last["n_instances"]
+        self._regularize()
+        return (loss, self.step.last["stats"], self.step.last["n_instances"],
+                self.grid_state.grid.grids.grad if self.grid_state is not None else None)
 
     def _set_inputs(self, w2c, cam_position, target, background):
         S = self.static
@@ -551,19 +666,13 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
         self._set_inputs(w2c, cam_position, target, background)
         if self.grid_state is not None:
             self.grid_state.set_image(image_idx)
+        if self.strategy is not None:
+            self.sh_degree = self.strategy.sh_degree
+            self.settings = dataclasses.replace(self.settings, active_sh_bases=(self.sh_degree + 1) ** 2)
         self.step.capacity = 0
         n = self.step.size_capacity(self.static["w2c"], self.settings, self.slack)
         self.capacity = self.step.capacity
-        self.dyn.zero_()  # warm-up iterations must not move the parameters: every group disabled
-        side = torch.cuda.Stream(self.dev)
-        side.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(side):
-            for _ in range(3):
-                self._body()
-        torch.cuda.current_stream(self.dev).wait_stream(side)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.loss, self.stats, self.n_isects = self._body()
+        self._warm_up_and_capture()
         return n
 
     def __call__(self, w2c, cam_position, target, background=None, image_idx=None):
@@ -573,6 +682,7 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
         self._set_inputs(w2c, cam_position, target, background)
         if self.grid_state is not None:
             self.grid_state.set_image(image_idx)
-        self._set_scalars()
-        self.graph.replay()
+        if self.strategy is None:
+            self._set_scalars()
+        self._replay()
         return self.loss

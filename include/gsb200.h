@@ -419,6 +419,68 @@ GSB_API int gsb_add_noise(uint32_t N, const float *raw_opacities, const float *r
                           const float *raw_quats, const float *noise, float *means, float current_lr,
                           gsb_stream_t stream);
 
+/* ---- SURVEY.md 8(f6): MCMC densification (src/training/strategies/mcmc.cpp:112-393, trainer.cpp:132-158) -------------
+ * All counts that depend on the data stay in DEVICE memory: a refine never synchronises with the host.  Indices are
+ * int32.  rotation_raw / raw_quats are read as float4: they must be 16-byte aligned (GSB_E_INVALID otherwise).  The four compute calls share one workspace of gsb_mcmc_workspace(N) bytes, 256-aligned.
+ *
+ * gsb_mcmc_dead: a Gaussian is dead when sigmoid(opacity_raw) <= min_opacity or |rotation_raw|^2 < 1e-8.  Writes the
+ *   ascending dead indices to dead_idx[0 .. *n_dead) (dead_idx holds N entries, *n_dead is a DEVICE uint32) and the
+ *   sampling weights: sigmoid(opacity_raw) where alive, 0 where dead.
+ * gsb_mcmc_sample: draws with replacement, weighted; sample j is the first i with C[i] > u_j * C[N-1], C the float64
+ *   inclusive prefix of the weights (or of sigmoid(weights) with weights_are_logits), so a zero weight is never drawn.
+ *   Draws min(n_samples, *n_samples_dev) samples (n_samples_dev: DEVICE uint32, nullable).  u_j in [0, 1) is
+ *   uniforms[j] (DEVICE float64, the test hook) or comes from the Philox state `philox` (torch's generator state; under
+ *   CUDA-graph capture its seed and offset are device pointers).  A sample is -1 when every weight is 0; a sample that
+ *   rounding of the prefix would put on a zero weight moves to the nearest positive one.
+ * gsb_mcmc_apply: targets non-NULL -- relocation (mcmc.cpp:112-190): sample j is copied onto row targets[j];
+ *   targets NULL -- growth (:192-347): onto row N + j (the caller's storage holds the rows).  ratio = min(copies of the
+ *   sample + 1, n_max) (binoms: [n_max][n_max] float), relocation's opacity clamped to [min_opacity, 1 - 1e-7]; the
+ *   sampled row and the target receive logit(opacity) and log(scale), the target a copy of means, sh0, shN and
+ *   rotation.  Adam moments: zeroed at the sampled rows when relocating (the targets keep theirs, as the reference's
+ *   update_optimizer_for_relocate does) and at the new rows when growing.  Samples < 0 are skipped. */
+typedef struct GsbPhilox {
+    uint64_t seed;
+    uint64_t offset;
+    const uint64_t *seed_ptr;   /* non-NULL under graph capture: the seed is read from the device */
+    const int64_t *offset_ptr;  /* non-NULL under graph capture: offset = *offset_ptr + offset_intragraph */
+    uint64_t offset_intragraph;
+} GsbPhilox;
+typedef struct GsbMcmcRows {
+    float *means;         /* [rows,3] */
+    float *sh0;           /* [rows,1,3] */
+    float *shN;           /* [rows,shN_rows,3]; NULL iff shN_rows == 0 */
+    float *scaling_raw;   /* [rows,3] */
+    float *rotation_raw;  /* [rows,4], 16-byte aligned */
+    float *opacity_raw;   /* [rows] */
+    uint32_t shN_rows;
+    /* Adam moments in the order means, sh0, shN, scaling_raw, rotation_raw, opacity_raw; NULL entries are skipped */
+    float *exp_avg[6];
+    float *exp_avg_sq[6];
+} GsbMcmcRows;
+GSB_API size_t gsb_mcmc_workspace(uint32_t N);
+GSB_API int gsb_mcmc_dead(uint32_t N, const float *opacity_raw, const float *rotation_raw, float min_opacity,
+                          int32_t *dead_idx, uint32_t *n_dead, float *weights, void *workspace, size_t workspace_bytes,
+                          gsb_stream_t stream);
+GSB_API int gsb_mcmc_sample(uint32_t N, const float *weights, int weights_are_logits, uint32_t n_samples,
+                            const uint32_t *n_samples_dev /*nullable*/, const double *uniforms /*nullable*/,
+                            const GsbPhilox *philox /*nullable iff uniforms*/, int32_t *samples, void *workspace,
+                            size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_mcmc_apply(uint32_t N, const GsbMcmcRows *rows, const int32_t *samples, uint32_t n_samples,
+                           const uint32_t *n_samples_dev /*nullable*/, const int32_t *targets /*NULL: growth*/,
+                           const float *binoms, int32_t n_max, float min_opacity, void *workspace,
+                           size_t workspace_bytes, gsb_stream_t stream);
+/* gsb_add_noise with the rate read on the device: current_lr = *lr * lr_scale (e.g. the means group's learning rate
+ * from the graphed step's scalars times the strategy's 5e5), so that the noise can be captured in a CUDA graph. */
+GSB_API int gsb_mcmc_add_noise(uint32_t N, const float *raw_opacities, const float *raw_scales,
+                               const float *raw_quats, const float *noise, float *means, const float *lr /*DEVICE*/,
+                               float lr_scale, gsb_stream_t stream);
+/* The trainer's regularisers: adds scale_reg * exp(s) / (3N) into v_scaling and opacity_reg * sigmoid(o) (1 -
+ * sigmoid(o)) / N into v_opacity (either nullable: that term is skipped) and writes loss_out (DEVICE float[2]) =
+ * (scale_reg * mean(exp(scaling_raw)), opacity_reg * mean(sigmoid(opacity_raw))).  Deterministic. */
+GSB_API int gsb_mcmc_regularize(uint32_t N, const float *scaling_raw, const float *opacity_raw, float scale_reg,
+                                float opacity_reg, float *v_scaling, float *v_opacity, float *loss_out,
+                                void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -95,4 +95,33 @@ void fused_adam_step_dynamic(const std::vector<at::Tensor> &params, const std::v
                              const std::vector<at::Tensor> &exp_avg, const std::vector<at::Tensor> &exp_avg_sq,
                              const at::Tensor dynamic_scalars, const double beta1, const double beta2, const double eps);
 
+// SURVEY.md 8 (f6): the MCMC strategy (src/training/strategies/mcmc.cpp) over the raw SplatData tensors, in place.
+// `params` are (means, sh0, shN, scaling_raw, rotation_raw, opacity_raw); exp_avg / exp_avg_sq their Adam moments in the
+// same order, or empty lists.  No operator reads a device value on the host.
+//
+// (dead_indices [N] int32, ascending in the first n_dead entries; n_dead [1] int32 on the device; weights [N]:
+// sigmoid(opacity_raw) where alive, 0 where dead) -- the dead mask of relocate_gs (mcmc.cpp:119-121).
+std::tuple<at::Tensor, at::Tensor, at::Tensor> mcmc_dead(const at::Tensor opacity_raw, const at::Tensor rotation_raw,
+                                                         const float min_opacity);
+// n_samples indices [n_samples] int32 drawn with replacement in proportion to weights (sigmoid(weights) when
+// weights_are_logits); only the first *n_samples_dev are drawn when it is given.  Uniforms from torch's default CUDA
+// generator (seeded by torch.manual_seed, graph-capturable) unless `uniforms` (float64) is given.
+at::Tensor mcmc_sample(const at::Tensor weights, const int64_t n_samples, const c10::optional<at::Tensor> n_samples_dev,
+                       const c10::optional<at::Tensor> uniforms, const bool weights_are_logits);
+// relocate_gs (mcmc.cpp:140-187) after the draw: sample j moves onto dead_indices[j], j < *n_dead
+void mcmc_relocate(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &exp_avg,
+                   const std::vector<at::Tensor> &exp_avg_sq, const at::Tensor samples, const at::Tensor dead_indices,
+                   const at::Tensor n_dead, const at::Tensor binoms, const float min_opacity);
+// add_new_gs (mcmc.cpp:213-344) after the draw: sample j is appended as row n_rows + j of storage that holds the rows
+void mcmc_grow(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &exp_avg,
+               const std::vector<at::Tensor> &exp_avg_sq, const int64_t n_rows, const at::Tensor samples,
+               const at::Tensor binoms, const float min_opacity);
+// inject_noise (mcmc.cpp:349-367) with the rate lr[0] * lr_scale read on the device
+void mcmc_add_noise(const at::Tensor raw_opacities, const at::Tensor raw_scales, const at::Tensor raw_quats,
+                    const at::Tensor noise, at::Tensor means, const at::Tensor lr, const float lr_scale);
+// trainer.cpp:132-158: gradients added into v_scaling / v_opacity; returns (scale loss, opacity loss) on the device
+at::Tensor mcmc_regularize(const at::Tensor scaling_raw, const at::Tensor opacity_raw, const float scale_reg,
+                           const float opacity_reg, c10::optional<at::Tensor> v_scaling,
+                           c10::optional<at::Tensor> v_opacity);
+
 } // namespace gsplat
