@@ -45,10 +45,11 @@ CUDA_SOURCES = [
     ("gsb_fastgs.cu", []),
     ("gsb_bilagrid.cu", []),
     ("gsb_mcmc.cu", []),
+    ("gsb_adc.cu", []),
 ]
 CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh",
                 "gsb_relocation.cuh"]
-SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
+SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "Adc.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
 
 
 def _run(cmd: list[str], verbose: bool) -> str:
@@ -131,6 +132,7 @@ def build_shim(verbose: bool = False, force: bool = False) -> str:
         incs += ["-I", i]
     hdrs = [os.path.join(INC, "gsb200.h")] + [os.path.join(INC, "gsplat", h) for h in ("Ops.h", "FusedOps.h", "Common.h", "Cameras.h")] + \
         [os.path.join(INC, "fastgs", "rasterization_api.h"), os.path.join(INC, "fastgs", "rasterization_ext.h"),
+         os.path.join(SHIM, "SplatRows.h"),
          os.path.join(INC, "kernels", "bilateral_grid.cuh")]
     def compile_one(src: str) -> str:
         sp = os.path.join(SHIM, src)

@@ -115,6 +115,15 @@ template <typename T> __host__ __device__ inline M3<T> rotmat_raw(T w, T x, T y,
     return r;
 }
 
+#ifdef __CUDACC__
+// normalised quaternion -> row-major rotation (Utils.cuh:80-102): gsb_quat_to_rotmat, add_noise and the ADC split
+__device__ __forceinline__ M3<float> quat_to_rotmat_norm(float w, float x, float y, float z, float max_inv_norm) {
+    float inv_norm = rsqrtf(x * x + y * y + z * z + w * w);
+    inv_norm = fminf(inv_norm, max_inv_norm);
+    return rotmat_raw(w * inv_norm, x * inv_norm, y * inv_norm, z * inv_norm);
+}
+#endif
+
 // Camera pose the way the reference derives it (gsplat/Cameras.cuh:33-71): the rotation block
 // of the row-major view matrix goes through a float quaternion (GLM quat_cast); t is column 3.
 struct CamPose {

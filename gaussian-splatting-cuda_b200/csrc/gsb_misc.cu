@@ -44,13 +44,7 @@ ProfScope::~ProfScope() {
 
 constexpr int kMiscThreads = 256;
 
-// normalised quaternion -> row-major rotation (Utils.cuh:80-102)
-__device__ __forceinline__ M3<float> quat_to_rotmat_norm(float w, float x, float y, float z, float max_inv_norm) {
-    float inv_norm = rsqrtf(x * x + y * y + z * z + w * w);
-    inv_norm = fminf(inv_norm, max_inv_norm);
-    return rotmat_raw(w * inv_norm, x * inv_norm, y * inv_norm, z * inv_norm);
-}
-
+// quat_to_rotmat_norm (gsb_common.cuh) is shared with the ADC split (gsb_adc.cu)
 __global__ void __launch_bounds__(kMiscThreads) quat_to_rotmat_kernel(uint32_t N, const float *__restrict__ quats,
                                                                        float *__restrict__ rotmats) {
     const uint32_t i = blockIdx.x * kMiscThreads + threadIdx.x;

@@ -8,7 +8,10 @@
                      the intersection buffer sized from a capacity so that the iteration has no host read-back
   strategy           optional MCMC densification (SURVEY.md 8 f6, mcmc.py): render -> loss -> backward -> regularisers
                      -> post_backward (SH bump, relocation / growth on refine iterations, noise) -> Adam (nothing to
-                     step on a growth iteration) -> scheduler
+                     step on a growth iteration) -> scheduler; or the default strategy (adc.py): the fastgs backward
+                     accumulates the strategy's statistics -> post_backward (SH bump, duplicate / split / prune on
+                     refine iterations, opacity reset) -> Adam (skipping the groups whose tensors were replaced or
+                     reset) -> scheduler
   bilateral_grid     optional (SURVEY.md 8 f5, trainer.cpp:662-665,698-705,758-762): render -> slice through the
                      image's grid -> unclamped loss -> + weight * TV of all grids -> backward -> one Adam launch for the
                      Gaussians and the grids (lr from the warm-up/exponential schedule, eps 1e-15)
@@ -23,6 +26,7 @@ from dataclasses import dataclass, field
 import torch
 
 from . import _product_ns, load, rasterize_fused
+from .adc import DefaultStrategy
 from .bilateral import BilateralGrid, WarmupExponentialLR
 from .mcmc import MCMC, growth_count
 
@@ -216,7 +220,7 @@ class TrainStep:
     bilateral_grid_lr: float = 2e-3
     tv_loss_weight: float = 10.0                 # mcmc_optimization_params.json (default_optimization_params.json: 5)
     grid_state: _GridState | None = None         # created on first use
-    strategy: MCMC | None = None                 # MCMC densification: owns params and the optimizer's moments
+    strategy: MCMC | DefaultStrategy | None = None  # densification: owns params and the optimizer's moments
 
     def __post_init__(self):
         _check_strategy(self.strategy, self.mcmc_noise_lr, self.params, self.optimizer, self.sh_degree)
@@ -290,18 +294,24 @@ def _check_strategy(strategy, mcmc_noise_lr: float, params=None, optimizer=None,
         raise ValueError("the step's optimizer must be the strategy's optimizer (growth replaces its moments)")
     if sh_degree is not None and int(sh_degree) != strategy.sh_degree:
         raise ValueError(f"sh_degree {sh_degree} differs from the strategy's active degree {strategy.sh_degree}: "
-                         "pass MCMC(..., sh_degree=...) or the step the same degree")
+                         f"pass {type(strategy).__name__}(..., sh_degree=...) or the step the same degree")
 
 
 def _strategy_post_backward(strategy, iteration: int):
     """Regularisers into the gradients, then the strategy's post_backward (trainer.cpp:668-756): on a growth iteration
-    the parameters become new leaves without gradients, so the following Adam step skips them."""
+    the parameters become new leaves without gradients, so the following Adam step skips them (the default strategy
+    also drops the opacity gradient after a reset)."""
     if strategy is None:
         return None
     with torch.no_grad():
         reg = strategy.regularize()
         strategy.post_backward(iteration)
     return reg
+
+
+def _densification_info(strategy):
+    """The default strategy's statistics tensor (empty after stop_refine); None for MCMC or no strategy."""
+    return strategy.densification_info if isinstance(strategy, DefaultStrategy) else None
 
 
 class GraphedTrainStep:
@@ -317,7 +327,8 @@ class GraphedTrainStep:
 
     def __init__(self, params: dict, sh_degree: int, width: int, height: int, cfg: AdamConfig | None = None,
                  lambda_dssim: float = 0.2, capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None,
-                 bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0, strategy: MCMC | None = None):
+                 bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0,
+                 strategy: MCMC | DefaultStrategy | None = None):
         load()
         _check_strategy(strategy, 0.0, params, None, sh_degree)
         self.params, self.sh_degree, self.W, self.H = params, int(sh_degree), int(width), int(height)
@@ -372,8 +383,8 @@ class GraphedTrainStep:
                 self.strategy.regularize()
 
     def _part_b(self, v_grids):
-        """[the strategy's noise at the means group's rate, read from `dyn` ->] Adam"""
-        if self.strategy is not None:
+        """[MCMC's noise at the means group's rate, read from `dyn` ->] Adam"""
+        if isinstance(self.strategy, MCMC):
             self.strategy.inject_noise(self.dyn[0, 0:1])
         self._adam(v_grids)
 
@@ -386,9 +397,12 @@ class GraphedTrainStep:
         """Warm-up iterations with every Adam group disabled and a zero noise rate (`dyn` is zero: nothing moves),
         then the capture.  Without a strategy the iteration is one graph.  With one it is two graphs -- (render, loss,
         backward, regularisers) and (noise, Adam) -- so that a refine can run eagerly between them, and the warm-up's
-        random draws are undone so that the replays draw what an eager run would."""
+        random draws are undone so that the replays draw what an eager run would.  The default strategy's statistics,
+        which the warm-up's backward passes accumulate into, are restored too."""
         self.dyn.zero_()
         rng = torch.cuda.get_rng_state(self.dev) if self.strategy is not None else None
+        info = _densification_info(self.strategy)
+        info_before = info.clone() if info is not None and info.numel() else None
         side = torch.cuda.Stream(self.dev)
         side.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(side):
@@ -401,6 +415,8 @@ class GraphedTrainStep:
             p.grad = None
         if rng is not None:
             torch.cuda.set_rng_state(rng, self.dev)
+        if info_before is not None:
+            info.copy_(info_before)
         self.graph = torch.cuda.CUDAGraph()
         self.captures += 1
         if self.strategy is None:
@@ -422,6 +438,9 @@ class GraphedTrainStep:
         if st is None:
             self.graph.replay()
             return
+        if isinstance(st, DefaultStrategy):
+            self._replay_default(st)
+            return
         lr0 = self.opt.lr[0]  # the rate before this iteration's scheduler step
         grows = st.is_refining(self.iteration) and growth_count(st.n, st.capacity) > 0
         self._set_scalars(skip_adam=grows)
@@ -433,6 +452,20 @@ class GraphedTrainStep:
         else:
             self.graph_b.replay()
         if grew or st.sh_degree != degree:
+            self.graph = None
+
+    def _replay_default(self, st: DefaultStrategy):
+        """Part A, then the eager post_backward, then the Adam scalars with the skipped groups disabled (their step
+        counts held), then part B.  A refine that replaced the tensors has nothing left to step: part B is not replayed
+        and the next call re-captures.  So does an SH-degree bump, and stop_refine, where the statistics the captured
+        backward writes go away.  A reset or a refine that changed nothing works in place and keeps the graphs."""
+        degree, info = st.sh_degree, st.densification_info
+        self.graph.replay()
+        skip = st.refine(self.iteration)
+        self._set_scalars(skip_groups=skip)
+        if not st.replaced:
+            self.graph_b.replay()
+        if st.replaced or st.sh_degree != degree or st.densification_info is not info:
             self.graph = None
 
     def _adam(self, v_grids=None):
@@ -473,14 +506,16 @@ class GraphedTrainStep:
         if background is not None:
             S["background"].copy_(background.reshape(1, 3), non_blocking=True)
 
-    def _set_scalars(self, skip_adam: bool = False):
+    def _set_scalars(self, skip_adam: bool = False, skip_groups: tuple = ()):
         """fused_adam.cpp:61-81 on the host: step counts, bias corrections, the shN freeze; strategy_utils.cpp:52-55 lr.
-        skip_adam: an iteration whose Adam step is skipped keeps the step counts (the learning rate still decays)."""
+        skip_adam: an iteration whose Adam step is skipped keeps the step counts (the learning rate still decays).
+        skip_groups: those groups are disabled and keep their step counts (a group without a gradient in FusedAdam)."""
         o = self.opt
         for i, k in enumerate(PARAM_GROUPS):
-            o.steps[k] += 0 if skip_adam else 1
+            skipped = skip_adam or k in skip_groups
+            o.steps[k] += 0 if skipped else 1
             t = o.steps[k]
-            enabled = 0.0 if (k == "shN" and self.iteration <= 1000) else 1.0
+            enabled = 0.0 if (k == "shN" and self.iteration <= 1000) or k in skip_groups else 1.0
             self.dyn_host[i, 0] = o.lr[i]
             self.dyn_host[i, 1] = 1.0 / (1.0 - o.cfg.beta1 ** t)
             self.dyn_host[i, 2] = 1.0 / math.sqrt(1.0 - o.cfg.beta2 ** t)
@@ -551,7 +586,7 @@ class FastGsTrainStep:
     tv_loss_weight: float = 10.0
     grid_state: _GridState | None = None         # created on first use
     index_on_device: bool = False                # the graphed wrapper refreshes grid_state.idx itself before each replay
-    strategy: MCMC | None = None                 # MCMC densification: owns params and the optimizer's moments
+    strategy: MCMC | DefaultStrategy | None = None  # densification: owns params and the optimizer's moments
 
     def __post_init__(self):
         _check_strategy(self.strategy, 0.0, self.params, self.optimizer, self.sh_degree)
@@ -582,6 +617,10 @@ class FastGsTrainStep:
         if self.strategy is not None:
             self.sh_degree = self.strategy.sh_degree
             settings = dataclasses.replace(settings, active_sh_bases=(self.sh_degree + 1) ** 2)
+        if isinstance(self.strategy, DefaultStrategy):  # the backward accumulates the strategy's statistics
+            if densification_info is not None:
+                raise ValueError("the default strategy owns densification_info: do not pass it as well")
+            densification_info = self.strategy.densification_info
         G = None
         if self.bilateral_grid is not None:
             G = self._grid()
@@ -630,7 +669,7 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
 
     def __init__(self, params: dict, sh_degree: int, settings, cfg: AdamConfig | None = None, lambda_dssim: float = 0.2,
                  capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None, bilateral_grid_lr: float = 2e-3,
-                 tv_loss_weight: float = 10.0, strategy: MCMC | None = None):
+                 tv_loss_weight: float = 10.0, strategy: MCMC | DefaultStrategy | None = None):
         super().__init__(params, sh_degree, settings.width, settings.height, cfg, lambda_dssim, capacity_slack,
                          bilateral_grid, bilateral_grid_lr, tv_loss_weight, strategy)
         from . import fastgs as fg
@@ -649,7 +688,8 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
     def _part_a(self):
         S = self.static
         self.step.capacity = self.capacity
-        loss = self.step(S["w2c"], self.settings, S["target"], S["background"])
+        loss = self.step(S["w2c"], self.settings, S["target"], S["background"],
+                         densification_info=_densification_info(self.strategy))
         self._regularize()
         return (loss, self.step.last["stats"], self.step.last["n_instances"],
                 self.grid_state.grid.grids.grad if self.grid_state is not None else None)

@@ -481,6 +481,49 @@ GSB_API int gsb_mcmc_regularize(uint32_t N, const float *scaling_raw, const floa
                                 float opacity_reg, float *v_scaling, float *v_opacity, float *loss_out,
                                 void *workspace, size_t workspace_bytes, gsb_stream_t stream);
 
+/* ---- Adaptive density control, the default densification strategy (src/training/strategies/default_strategy.cpp:
+ * 164-290) --------------------------------------------------------------------------------------------------------------
+ * A refine -- grow_gs (duplicate, then split) followed by prune_gs -- is one compaction into freshly allocated rows:
+ *   gsb_adc_classify: per row, with g = info[1] / max(info[0], 1) (densification_info [2,N]; NULL: no row is high):
+ *     duplicate = g > grad_threshold and max(exp(scaling_raw)) <= grow_scale3d * scene_scale; split = g >
+ *     grad_threshold and not small.  prune_gs then removes a row (original, duplicate copy or split copy) when
+ *     sigmoid(opacity_raw) < prune_opacity, |rotation_raw|^2 < 1e-8 or, when prune_too_big, max(exp(scaling_raw)) >
+ *     prune_scale3d * scene_scale.  Writes counts (DEVICE int32[8]): [0] duplicated, [1] split, [2] pruned from the
+ *     grown set, [3] final rows, [4..6] kept rest rows / duplicate copies / split rows, [7] 0.  The flags and ranks stay
+ *     in the workspace for gsb_adc_apply.  N must be at most INT32_MAX / 2 (the grown set of N + n_dup + n_split <= 2N
+ *     rows is indexed in int32).
+ *   gsb_adc_apply: writes the final rows into dst (which holds n_final = counts[3] rows; n_split = counts[1], both read
+ *     back by the caller) in the reference's order: kept rows that were not split, kept duplicate copies, copy 0 of
+ *     every kept split row, copy 1 of every kept split row.  Copy b of split row i takes means + R(normalize(q))
+ *     (exp(scaling_raw) * z[b, rank of i among split rows]) (z: [2, n_split, 3], torch::randn's draw), scaling_raw =
+ *     log(exp(scaling_raw) * (1.0f / 1.6f)) and, with revised_opacity, opacity_raw = logit(1 - sqrt(1 -
+ *     sigmoid(opacity_raw))).  Adam moments: copied for kept original rows, zero for new rows (NULL entries skipped).
+ *     densification_info (nullable) receives zeros [2, n_final].  Same workspace and params as the classify call.
+ *   gsb_adc_reset_opacity: opacity_raw = min(opacity_raw, logit(2 prune_opacity)) (the logit in float), the opacity
+ *     group's moments (nullable) zeroed.
+ * rotation_raw is read as float4: 16-byte aligned (GSB_E_INVALID otherwise).  Workspace: gsb_adc_workspace(N) bytes,
+ * 256-aligned. */
+typedef struct GsbAdcParams {
+    float grad_threshold;
+    float grow_scale3d;
+    float prune_scale3d;
+    float scene_scale;
+    float prune_opacity;
+    int32_t prune_too_big;   /* iter > reset_every */
+    int32_t revised_opacity;
+} GsbAdcParams;
+GSB_API size_t gsb_adc_workspace(uint32_t N);
+GSB_API int gsb_adc_classify(uint32_t N, const float *densification_info /*nullable*/, const float *scaling_raw,
+                             const float *rotation_raw, const float *opacity_raw, const GsbAdcParams *params,
+                             int32_t *counts /*DEVICE [8]*/, void *workspace, size_t workspace_bytes,
+                             gsb_stream_t stream);
+GSB_API int gsb_adc_apply(uint32_t N, const GsbMcmcRows *src, const GsbMcmcRows *dst, uint32_t n_split,
+                          uint32_t n_final, const float *z /*nullable iff n_split == 0*/, const GsbAdcParams *params,
+                          const int32_t *counts /*DEVICE, from gsb_adc_classify*/, float *densification_info /*nullable*/,
+                          void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_adc_reset_opacity(uint32_t N, float *opacity_raw, float prune_opacity, float *exp_avg /*nullable*/,
+                                  float *exp_avg_sq /*nullable*/, gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -124,4 +124,27 @@ at::Tensor mcmc_regularize(const at::Tensor scaling_raw, const at::Tensor opacit
                            const float opacity_reg, c10::optional<at::Tensor> v_scaling,
                            c10::optional<at::Tensor> v_opacity);
 
+// Adaptive density control, the default strategy (src/training/strategies/default_strategy.cpp:164-290).  A refine is
+// adc_classify then adc_apply; between them the caller reads counts back once (the output size and the shape of
+// torch::randn({2, n_split, 3})).
+//
+// grow_gs and prune_gs classified per row: (counts [8] int32 on the device -- duplicated, split, pruned, final rows,
+// kept rest rows, kept duplicate copies, kept split rows, 0 -- and the workspace that adc_apply reads).  An undefined or
+// empty densification_info means no row is high (nothing grows).  prune_too_big: iter > reset_every.
+std::tuple<at::Tensor, at::Tensor> adc_classify(const at::Tensor densification_info, const at::Tensor scaling_raw,
+                                                const at::Tensor rotation_raw, const at::Tensor opacity_raw,
+                                                const float grad_threshold, const float grow_scale3d,
+                                                const float prune_scale3d, const float scene_scale,
+                                                const float prune_opacity, const bool prune_too_big,
+                                                const bool revised_opacity);
+// The final (params, exp_avg, exp_avg_sq, zeroed densification_info [2, n_final]) in freshly allocated tensors, rows in
+// the reference's order; n_split = counts[1], n_final = counts[3]; z = torch::randn({2, n_split, 3}).
+std::tuple<std::vector<at::Tensor>, std::vector<at::Tensor>, std::vector<at::Tensor>, at::Tensor>
+adc_apply(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &exp_avg,
+          const std::vector<at::Tensor> &exp_avg_sq, const at::Tensor workspace, const at::Tensor counts,
+          const int64_t n_split, const int64_t n_final, const c10::optional<at::Tensor> z, const bool revised_opacity);
+// reset_opacity (:251-290) in place: opacity_raw = min(opacity_raw, logit(2 prune_opacity)), its moments zeroed
+void adc_reset_opacity(at::Tensor opacity_raw, c10::optional<at::Tensor> exp_avg, c10::optional<at::Tensor> exp_avg_sq,
+                       const float prune_opacity);
+
 } // namespace gsplat
