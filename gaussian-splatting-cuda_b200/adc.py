@@ -25,6 +25,18 @@ from . import _product_ns, load
 PARAM_GROUPS = ("means", "sh0", "shN", "scaling_raw", "rotation_raw", "opacity_raw")
 
 
+def lowest_opacity_removed(params: list, exp_avg: list, exp_avg_sq: list, n_prune: int):
+    """The rows of the six tensors and their moments (PARAM_GROUPS order) without the n_prune rows of lowest
+    sigmoid(opacity_raw), in order, in freshly allocated tensors: (params, exp_avg, exp_avg_sq, zeroed statistics
+    [2, n_kept]).  The sparsifier's final prune (sparsity_optimizer.cpp:104-143 + remove_gaussians); n_prune and the
+    row count are known on the host, so nothing is read back."""
+    ns = _product_ns()
+    n = int(params[0].shape[0])
+    with torch.no_grad():
+        counts, ws = ns.sparsity_prune_classify(params[5].reshape(-1), n_prune)
+        return ns.adc_apply(params, exp_avg, exp_avg_sq, ws, counts, 0, n - n_prune, None, False)
+
+
 @dataclass
 class DefaultConfig:
     """parameter/default_optimization_params.json (the fields the strategy is given; values already scaled by
@@ -122,6 +134,19 @@ class DefaultStrategy:
             opt.exp_avg[k], opt.exp_avg_sq[k] = m1, m2
         self.densification_info = new_info
         return True
+
+    def remove_lowest_opacity(self, n_prune: int) -> None:
+        """remove_gaussians (default_strategy.cpp:194-227) of the n_prune lowest-opacity rows: new tensors and
+        moments, step counts kept.  Non-empty statistics become zeros [2, n_kept]."""
+        P, opt = self.params, self.optimizer
+        out_p, out_m1, out_m2, new_info = lowest_opacity_removed(
+            [P[k].detach() for k in PARAM_GROUPS], [opt.exp_avg[k] for k in PARAM_GROUPS],
+            [opt.exp_avg_sq[k] for k in PARAM_GROUPS], n_prune)
+        for k, p, m1, m2 in zip(PARAM_GROUPS, out_p, out_m1, out_m2):
+            P[k] = p.requires_grad_(True)
+            opt.exp_avg[k], opt.exp_avg_sq[k] = m1, m2
+        if self.densification_info.numel():
+            self.densification_info = new_info
 
     def reset_opacity(self) -> None:
         """default_strategy.cpp:251-290 in place."""

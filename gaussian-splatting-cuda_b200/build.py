@@ -46,10 +46,12 @@ CUDA_SOURCES = [
     ("gsb_bilagrid.cu", []),
     ("gsb_mcmc.cu", []),
     ("gsb_adc.cu", []),
+    ("gsb_sparsity.cu", []),
 ]
 CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh",
-                "gsb_relocation.cuh"]
-SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "Adc.cpp", "torch_binding.cpp", "fastgs_binding.cpp"]
+                "gsb_relocation.cuh", "gsb_select.cuh"]
+SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "Adc.cpp", "Sparsity.cpp", "torch_binding.cpp",
+                "fastgs_binding.cpp"]
 
 
 def _run(cmd: list[str], verbose: bool) -> str:

@@ -18,11 +18,15 @@
 //                     236 parameter bytes per row at degree 3) is read and written by consecutive threads.  New rows
 //                     get zero moments.
 //   gsb_adc_reset_opacity   opacity_raw = min(opacity_raw, logit(2 prune_opacity)) in place, the group's moments zeroed.
+//   gsb_adc_prune_classify  the ADMM sparsifier's final prune as flags and ranks for gsb_adc_apply: the n_prune-th
+//                     smallest sigmoid(opacity_raw) v by gsb_select.cuh's device select, every row below v removed,
+//                     rows equal to v removed in index order until n_prune rows are gone (one scan ranks the ties).
 // No fast-math: the flags compare exp / log / sigmoid values with thresholds, bit for bit as torch computes them.
 #include <cmath>
 
 #include "gsb_common.cuh"
 #include "gsb_devsort.cuh"
+#include "gsb_select.cuh"
 
 namespace gsb {
 namespace adc {
@@ -106,8 +110,7 @@ static Thresholds thresholds(const GsbAdcParams &p) {
             p.prune_too_big != 0, p.revised_opacity != 0};
 }
 
-// torch's float sigmoid / logit on CUDA (IEEE expf / logf)
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
+// torch's float logit on CUDA (IEEE logf); sigmoid_f is gsb_common.cuh's
 __device__ __forceinline__ float logit_f(float x) { return logf(x / (1.0f - x)); }
 // torch::max over the last dim propagates NaN
 __device__ __forceinline__ float max_nan(float a, float b) { return (a > b || a != a) ? a : b; }
@@ -288,6 +291,54 @@ __global__ void __launch_bounds__(kThreads) reset_opacity_kernel(uint32_t N, flo
     o[i] = v > thr ? thr : v; // torch::clamp_max: NaN stays
 }
 
+// ---- the sparsifier's final prune (gsb_adc_prune_classify) --------------------------------------------------------
+// Workspace reuse: the keys live in `map` (written by gsb_adc_apply only), the select's histograms in `bsum` (before
+// the scan uses it), its state in the 256-byte head.
+static_assert(sel::kHistBytes <= kScanBlocks * sizeof(Cnt4), "the select histograms must fit the scan's block sums");
+static_assert(sizeof(sel::SelectState) <= 256, "the select state must fit the workspace head");
+
+__global__ void __launch_bounds__(kThreads) prune_keys_kernel(uint32_t N, const float *__restrict__ opacity_raw,
+                                                              uint32_t *__restrict__ keys) {
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i < N) keys[i] = sel::float_key(sigmoid_f(opacity_raw[i]));
+}
+
+// below the n_prune-th smallest key: pruned; equal to it: a tie (kSplit marks it for the scan); above: kept
+__global__ void __launch_bounds__(kThreads) prune_flags_kernel(uint32_t N, const uint32_t *__restrict__ keys,
+                                                               const sel::SelectState *__restrict__ st, bool none,
+                                                               uint8_t *__restrict__ flags) {
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i >= N) return;
+    if (none) {
+        flags[i] = kKeepRest;
+        return;
+    }
+    const uint32_t k = keys[i], v = st->prefix;
+    flags[i] = k > v ? kKeepRest : (k == v ? kSplit : 0);
+}
+
+// After the scan (split = rank among ties, rest = rank among rows above the boundary): the first n_prune - n_less
+// ties in index order are pruned, the others kept, and every kept row's rank becomes its rank among all kept rows.
+__global__ void __launch_bounds__(kThreads) prune_ranks_kernel(uint32_t N, uint32_t n_prune,
+                                                               const sel::SelectState *__restrict__ st, bool none,
+                                                               uint8_t *__restrict__ flags, Cnt4 *__restrict__ ranks,
+                                                               int32_t *__restrict__ counts) {
+    const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+    if (i == 0) {
+        const int32_t kept = (int32_t)(N - n_prune);
+        counts[0] = 0; counts[1] = 0; counts[2] = (int32_t)n_prune; counts[3] = kept;
+        counts[4] = kept; counts[5] = 0; counts[6] = 0; counts[7] = 0;
+    }
+    if (i >= N || none) return;
+    const int32_t tie_pruned = (int32_t)(n_prune - st->n_less);
+    const uint8_t f = flags[i];
+    Cnt4 r = ranks[i];
+    const int32_t kept_ties = r.split > tie_pruned ? r.split - tie_pruned : 0;
+    if (f & kSplit) flags[i] = r.split > tie_pruned ? kKeepRest : 0;
+    r.rest += kept_ties;
+    ranks[i] = r;
+}
+
 static unsigned blocks_for(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 static bool rows_valid(const GsbMcmcRows &r) {
@@ -363,6 +414,46 @@ extern "C" int gsb_adc_apply(uint32_t N, const GsbMcmcRows *src, const GsbMcmcRo
         shn_kernel<<<(n_final + kShnRowsPerBlock - 1) / kShnRowsPerBlock, kThreads, 0, s>>>(a);
         GSB_LAUNCH_CHECK();
     }
+    return GSB_OK;
+}
+
+extern "C" int gsb_adc_prune_classify(uint32_t N, const float *opacity_raw, uint32_t n_prune, int32_t *counts,
+                                      void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    using namespace gsb::adc;
+    if (!counts || n_prune > N) return GSB_E_INVALID;
+    if ((uint64_t)N * 2 > (uint64_t)INT32_MAX) return GSB_E_INVALID; // gsb_adc_apply's bound
+    cudaStream_t s = as_stream(stream);
+    if (N == 0) {
+        GSB_CUDA_TRY(cudaMemsetAsync(counts, 0, 8 * sizeof(int32_t), s));
+        return GSB_OK;
+    }
+    if (!opacity_raw) return GSB_E_INVALID;
+    Ws w;
+    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    uint32_t *keys = w.map;
+    uint32_t *hist = reinterpret_cast<uint32_t *>(w.bsum);
+    sel::SelectState *st = static_cast<sel::SelectState *>(workspace);
+    const bool none = n_prune == 0;
+    ProfScope ps("adc_prune_classify", s);
+    GSB_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(sel::SelectState), s));
+    if (!none) {
+        prune_keys_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, opacity_raw, keys);
+        GSB_LAUNCH_CHECK();
+        if (int rc = sel::select_kth(keys, N, n_prune, hist, st, s)) return rc;
+    }
+    prune_flags_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, keys, st, none, w.flags);
+    GSB_LAUNCH_CHECK();
+    uint64_t nb = (N + 4095) / 4096;
+    if (nb > kScanBlocks) nb = kScanBlocks;
+    const uint32_t seg = (uint32_t)((N + nb - 1) / nb);
+    const LoadFlags load{w.flags};
+    scan_blocksum_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum);
+    GSB_LAUNCH_CHECK();
+    scan_apply_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum, w.ranks);
+    GSB_LAUNCH_CHECK();
+    prune_ranks_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, n_prune, st, none, w.flags, w.ranks, counts);
+    GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
 

@@ -122,6 +122,9 @@ __device__ __forceinline__ M3<float> quat_to_rotmat_norm(float w, float x, float
     inv_norm = fminf(inv_norm, max_inv_norm);
     return rotmat_raw(w * inv_norm, x * inv_norm, y * inv_norm, z * inv_norm);
 }
+
+// torch's float sigmoid on CUDA (IEEE expf, no fast-math): the ADC flags and the sparsifier compare its values
+__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 #endif
 
 // Camera pose the way the reference derives it (gsplat/Cameras.cuh:33-71): the rotation block

@@ -132,6 +132,22 @@ class MCMC:
         self._views()
         return n_new
 
+    def remove_lowest_opacity(self, n_prune: int) -> None:
+        """remove_gaussians (mcmc.cpp:404-440) of the n_prune lowest-opacity rows: the kept rows are compacted into
+        fresh rows (the compaction must not read and write the same rows), written back to the front of the storage,
+        and the views re-created.  Step counts are kept."""
+        from .adc import lowest_opacity_removed
+        p, m1, m2 = self._lists(self.n)
+        out_p, out_m1, out_m2, _ = lowest_opacity_removed(p, m1, m2, n_prune)
+        kept = self.n - n_prune
+        with torch.no_grad():
+            for k, a, b, c in zip(PARAM_GROUPS, out_p, out_m1, out_m2):
+                self.store[k][:kept].copy_(a)
+                self.store_m1[k][:kept].copy_(b)
+                self.store_m2[k][:kept].copy_(c)
+        self.n = kept
+        self._views()
+
     def inject_noise(self, lr: float | torch.Tensor) -> None:
         """inject_noise (mcmc.cpp:349-367): lr is group 0's learning rate, a float or a device scalar."""
         P = self.params

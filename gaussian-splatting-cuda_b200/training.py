@@ -15,6 +15,9 @@
   bilateral_grid     optional (SURVEY.md 8 f5, trainer.cpp:662-665,698-705,758-762): render -> slice through the
                      image's grid -> unclamped loss -> + weight * TV of all grids -> backward -> one Adam launch for the
                      Gaussians and the grids (lr from the warm-up/exponential schedule, eps 1e-15)
+  sparsity           optional ADMM sparsification with a strategy (sparsity.py, trainer.cpp:173-247,707-784): after
+                     the regularisers the sparsity loss's gradient; post_backward only up to the base iteration count;
+                     after Adam the state update and, on the last iteration, the prune
 
 Everything that computes lives behind the C ABI; this file only orders the calls, like the reference's trainer does."""
 from __future__ import annotations
@@ -29,6 +32,7 @@ from . import _product_ns, load, rasterize_fused
 from .adc import DefaultStrategy
 from .bilateral import BilateralGrid, WarmupExponentialLR
 from .mcmc import MCMC, growth_count
+from .sparsity import ADMMSparsity
 
 
 class _PhotometricLoss(torch.autograd.Function):
@@ -221,9 +225,11 @@ class TrainStep:
     tv_loss_weight: float = 10.0                 # mcmc_optimization_params.json (default_optimization_params.json: 5)
     grid_state: _GridState | None = None         # created on first use
     strategy: MCMC | DefaultStrategy | None = None  # densification: owns params and the optimizer's moments
+    sparsity: ADMMSparsity | None = None            # ADMM sparsification after the base iterations (needs a strategy)
 
     def __post_init__(self):
         _check_strategy(self.strategy, self.mcmc_noise_lr, self.params, self.optimizer, self.sh_degree)
+        _check_sparsity(self.sparsity, self.strategy)
 
     def _grid(self) -> _GridState:
         if self.grid_state is None:
@@ -252,7 +258,9 @@ class TrainStep:
             loss.backward()
             G.grid.grids.grad = v_grids
             loss = loss.detach() + G.weight[0] * tv  # the trainer's loss_value includes the TV term
-        reg = _strategy_post_backward(self.strategy, self.iteration)
+        reg, sp_loss = _post_backward(self.strategy, self.sparsity, self.iteration)
+        if sp_loss is not None:
+            loss = loss.detach() + sp_loss[0]
         if self.optimizer is not None:
             if self.bilateral_grid is not None:
                 extra = self.grid_state.adam_group()
@@ -266,7 +274,9 @@ class TrainStep:
             self.optimizer.zero_grad()
         if self.bilateral_grid is not None:
             self.bilateral_grid.grids.grad = None
-        self.last = {"n_isects": out.n_isects, "stats": stats, "reg": reg}
+        if self.sparsity is not None:
+            self.sparsity.after_step(self.strategy, self.iteration)
+        self.last = {"n_isects": out.n_isects, "stats": stats, "reg": reg, "sparsity_loss": sp_loss}
         return loss
 
     def size_capacity(self, viewmat, K, target, background=None, slack: float = 1.25):
@@ -309,6 +319,25 @@ def _strategy_post_backward(strategy, iteration: int):
     return reg
 
 
+def _check_sparsity(sparsity, strategy) -> None:
+    if sparsity is not None and strategy is None:
+        raise ValueError("sparsity needs a strategy: the final prune removes rows from the strategy's tensors, and "
+                         "the strategy's post_backward stops after the base iterations")
+
+
+def _post_backward(strategy, sparsity, iteration: int):
+    """(regulariser losses, sparsity loss): the regularisers, the sparsity loss's gradient when it applies
+    (trainer.cpp:707-714), then the strategy's post_backward up to the base iteration count (trainer.cpp:745-754)."""
+    if sparsity is None:
+        return _strategy_post_backward(strategy, iteration), None
+    with torch.no_grad():
+        reg = strategy.regularize()
+        sp = sparsity.loss_step(strategy.params["opacity_raw"], iteration)
+        if sparsity.post_backward_due(iteration):
+            strategy.post_backward(iteration)
+    return reg, sp
+
+
 def _densification_info(strategy):
     """The default strategy's statistics tensor (empty after stop_refine); None for MCMC or no strategy."""
     return strategy.densification_info if isinstance(strategy, DefaultStrategy) else None
@@ -328,9 +357,12 @@ class GraphedTrainStep:
     def __init__(self, params: dict, sh_degree: int, width: int, height: int, cfg: AdamConfig | None = None,
                  lambda_dssim: float = 0.2, capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None,
                  bilateral_grid_lr: float = 2e-3, tv_loss_weight: float = 10.0,
-                 strategy: MCMC | DefaultStrategy | None = None):
+                 strategy: MCMC | DefaultStrategy | None = None, sparsity: ADMMSparsity | None = None):
         load()
         _check_strategy(strategy, 0.0, params, None, sh_degree)
+        _check_sparsity(sparsity, strategy)
+        self.sparsity = sparsity
+        self.sparsity_in_graph = False  # the captured part A adds the sparsity loss (part B then has no MCMC noise)
         self.params, self.sh_degree, self.W, self.H = params, int(sh_degree), int(width), int(height)
         self.lambda_dssim = float(lambda_dssim)
         # with a strategy, its optimizer (whose moments live in the strategy's storage) is the step's
@@ -367,24 +399,28 @@ class GraphedTrainStep:
         if self.grid_state is None:
             loss, stats = photometric_loss(out.render_colors, S["target"], self.lambda_dssim)
             loss.backward()
-            self._regularize()
-            return loss, stats, out.n_isects, None
+            return self._regularize(loss), stats, out.n_isects, None
         G = self.grid_state
         tv, v_grids = G.tv()
         sliced = _SliceIntoGrad.apply(out.render_colors, G.grid.grids.detach(), G.idx, v_grids, False)
         loss, stats = photometric_loss_unclamped(sliced, S["target"], self.lambda_dssim)
         loss.backward()
-        self._regularize()
-        return loss.detach() + G.weight[0] * tv, stats, out.n_isects, v_grids
+        return self._regularize(loss.detach() + G.weight[0] * tv), stats, out.n_isects, v_grids
 
-    def _regularize(self):
+    def _regularize(self, loss):
+        """The strategy's regularisers, then, in the sparsity phase, the sparsity loss (rho read on the device: zero
+        on the prune iteration).  Returns the iteration's loss."""
         if self.strategy is not None:
             with torch.no_grad():
                 self.strategy.regularize()
+                if self.sparsity_in_graph:
+                    return loss.detach() + self.sparsity.add_loss_gradient(self.params["opacity_raw"])[0]
+        return loss
 
     def _part_b(self, v_grids):
-        """[MCMC's noise at the means group's rate, read from `dyn` ->] Adam"""
-        if isinstance(self.strategy, MCMC):
+        """[MCMC's noise at the means group's rate, read from `dyn` ->] Adam.  In the sparsity phase the strategy's
+        post_backward, and with it the noise, stops: part B is Adam only."""
+        if isinstance(self.strategy, MCMC) and not self.sparsity_in_graph:
             self.strategy.inject_noise(self.dyn[0, 0:1])
         self._adam(v_grids)
 
@@ -400,6 +436,8 @@ class GraphedTrainStep:
         random draws are undone so that the replays draw what an eager run would.  The default strategy's statistics,
         which the warm-up's backward passes accumulate into, are restored too."""
         self.dyn.zero_()
+        sp = self.sparsity
+        self.sparsity_in_graph = sp is not None and sp.initialized and not sp.done
         rng = torch.cuda.get_rng_state(self.dev) if self.strategy is not None else None
         info = _densification_info(self.strategy)
         info_before = info.clone() if info is not None and info.numel() else None
@@ -438,35 +476,59 @@ class GraphedTrainStep:
         if st is None:
             self.graph.replay()
             return
+        sp = self.sparsity
+        post = sp is None or sp.post_backward_due(self.iteration)  # no post_backward after the base iterations
         if isinstance(st, DefaultStrategy):
-            self._replay_default(st)
-            return
+            self._replay_default(st, post)
+        else:
+            self._replay_mcmc(st, post)
+        if sp is not None and sp.after_step(st, self.iteration):  # the prune replaced the tensors
+            self.graph = None
+
+    def _replay_mcmc(self, st: MCMC, post: bool):
         lr0 = self.opt.lr[0]  # the rate before this iteration's scheduler step
-        grows = st.is_refining(self.iteration) and growth_count(st.n, st.capacity) > 0
+        grows = post and st.is_refining(self.iteration) and growth_count(st.n, st.capacity) > 0
         self._set_scalars(skip_adam=grows)
         degree = st.sh_degree
         self.graph.replay()
-        grew = st.refine(self.iteration)
+        grew = st.refine(self.iteration) if post else False
         if grew:
             st.inject_noise(lr0)
         else:
+            if post and self.sparsity_in_graph:  # the base iteration: its noise is no longer in part B
+                st.inject_noise(lr0)
             self.graph_b.replay()
         if grew or st.sh_degree != degree:
             self.graph = None
 
-    def _replay_default(self, st: DefaultStrategy):
+    def _replay_default(self, st: DefaultStrategy, post: bool = True):
         """Part A, then the eager post_backward, then the Adam scalars with the skipped groups disabled (their step
         counts held), then part B.  A refine that replaced the tensors has nothing left to step: part B is not replayed
         and the next call re-captures.  So does an SH-degree bump, and stop_refine, where the statistics the captured
         backward writes go away.  A reset or a refine that changed nothing works in place and keeps the graphs."""
         degree, info = st.sh_degree, st.densification_info
         self.graph.replay()
-        skip = st.refine(self.iteration)
+        skip = st.refine(self.iteration) if post else ()
+        replaced = post and st.replaced
         self._set_scalars(skip_groups=skip)
-        if not st.replaced:
+        if not replaced:
             self.graph_b.replay()
-        if st.replaced or st.sh_degree != degree or st.densification_info is not info:
+        if replaced or st.sh_degree != degree or st.densification_info is not info:
             self.graph = None
+
+    def _enter_iteration(self) -> None:
+        """Before the capture check of iteration self.iteration + 1: the sparsifier's lazy initialisation at its first
+        loss iteration, which re-captures part A with the loss in it; rho set to zero where no loss applies."""
+        sp = self.sparsity
+        if sp is None or sp.done:
+            return
+        it = self.iteration + 1
+        sp.check_rows(self.strategy.n)
+        if sp.should_apply_loss(it) and not sp.initialized:
+            sp.initialize(self.params["opacity_raw"])
+            self.graph = None
+        if sp.initialized and not sp.should_apply_loss(it):  # the prune iteration
+            sp.rho.zero_()
 
     def _adam(self, v_grids=None):
         """One launch for the Gaussians' groups (and the grids' after them), scalars from `dyn`."""
@@ -548,6 +610,7 @@ class GraphedTrainStep:
         return n
 
     def __call__(self, viewmat, K, target, background=None, image_idx=None):
+        self._enter_iteration()
         if self.graph is None:
             self.capture(viewmat, K, target, background, image_idx)
         self.iteration += 1
@@ -587,9 +650,11 @@ class FastGsTrainStep:
     grid_state: _GridState | None = None         # created on first use
     index_on_device: bool = False                # the graphed wrapper refreshes grid_state.idx itself before each replay
     strategy: MCMC | DefaultStrategy | None = None  # densification: owns params and the optimizer's moments
+    sparsity: ADMMSparsity | None = None            # ADMM sparsification after the base iterations (needs a strategy)
 
     def __post_init__(self):
         _check_strategy(self.strategy, 0.0, self.params, self.optimizer, self.sh_degree)
+        _check_sparsity(self.sparsity, self.strategy)
 
     def _grid(self) -> _GridState:
         if self.grid_state is None:
@@ -650,15 +715,19 @@ class FastGsTrainStep:
                             P["shN"], w2c, settings, densification_info)
             for k, gk in zip(("means", "scaling_raw", "rotation_raw", "opacity_raw", "sh0", "shN"), g[:6]):
                 P[k].grad = gk.reshape(P[k].shape)
-        reg = _strategy_post_backward(self.strategy, self.iteration)
+        reg, sp_loss = _post_backward(self.strategy, self.sparsity, self.iteration)
         if self.optimizer is not None:
             self.optimizer.step(self.iteration, G.adam_group() if G is not None else None)
             self.optimizer.zero_grad()
             if G is not None:
                 G.grid.grids.grad = None
+        if self.sparsity is not None:
+            self.sparsity.after_step(self.strategy, self.iteration)
         # capacity mode: the count is a device tensor (compare it with the capacity when convenient)
-        self.last = {"n_instances": ctx.get("n_instances_dev", int(ctx["ints"][1])), "stats": stats, "reg": reg}
-        return stats[0] if G is None else stats[0] + G.weight[0] * tv
+        self.last = {"n_instances": ctx.get("n_instances_dev", int(ctx["ints"][1])), "stats": stats, "reg": reg,
+                     "sparsity_loss": sp_loss}
+        loss = stats[0] if G is None else stats[0] + G.weight[0] * tv
+        return loss if sp_loss is None else loss + sp_loss[0]
 
 
 class GraphedFastGsTrainStep(GraphedTrainStep):
@@ -669,9 +738,10 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
 
     def __init__(self, params: dict, sh_degree: int, settings, cfg: AdamConfig | None = None, lambda_dssim: float = 0.2,
                  capacity_slack: float = 1.25, bilateral_grid: BilateralGrid | None = None, bilateral_grid_lr: float = 2e-3,
-                 tv_loss_weight: float = 10.0, strategy: MCMC | DefaultStrategy | None = None):
+                 tv_loss_weight: float = 10.0, strategy: MCMC | DefaultStrategy | None = None,
+                 sparsity: ADMMSparsity | None = None):
         super().__init__(params, sh_degree, settings.width, settings.height, cfg, lambda_dssim, capacity_slack,
-                         bilateral_grid, bilateral_grid_lr, tv_loss_weight, strategy)
+                         bilateral_grid, bilateral_grid_lr, tv_loss_weight, strategy, sparsity)
         from . import fastgs as fg
         dev = self.dev
         self.static = {"w2c": torch.zeros((4, 4), device=dev), "campos": torch.zeros((3,), device=dev),
@@ -690,7 +760,7 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
         self.step.capacity = self.capacity
         loss = self.step(S["w2c"], self.settings, S["target"], S["background"],
                          densification_info=_densification_info(self.strategy))
-        self._regularize()
+        loss = self._regularize(loss)
         return (loss, self.step.last["stats"], self.step.last["n_instances"],
                 self.grid_state.grid.grids.grad if self.grid_state is not None else None)
 
@@ -716,6 +786,7 @@ class GraphedFastGsTrainStep(GraphedTrainStep):
         return n
 
     def __call__(self, w2c, cam_position, target, background=None, image_idx=None):
+        self._enter_iteration()
         if self.graph is None:
             self.capture(w2c, cam_position, target, background, image_idx)
         self.iteration += 1

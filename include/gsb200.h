@@ -524,6 +524,31 @@ GSB_API int gsb_adc_apply(uint32_t N, const GsbMcmcRows *src, const GsbMcmcRows 
 GSB_API int gsb_adc_reset_opacity(uint32_t N, float *opacity_raw, float prune_opacity, float *exp_avg /*nullable*/,
                                   float *exp_avg_sq /*nullable*/, gsb_stream_t stream);
 
+/* ---- ADMM opacity sparsification (src/training/components/sparsity_optimizer.cpp) ------------------------------------
+ * s = sigmoid(opacity_raw) in float; k = (int)(prune_ratio * N) as the caller forms it (a float product); prune_z(x) =
+ * (x > x_(k)) * x with x_(k) the k-th smallest of x (NaN sorts last), and 0 when k == 0.  The k-th value is found by
+ * radix passes on the device and never read back: every call below is stream-ordered and graph-capturable.
+ *   gsb_sparsity_update: initialize != 0: u = 0, z = prune_z(s + u); otherwise zt = s + u, z = prune_z(zt),
+ *     u += s - z.  z, u: [N] float, bit for bit as torch computes them.  k must be at most N.
+ *   gsb_sparsity_loss: loss_out (DEVICE float[1]) = 0.5 * rho * ||s - z + u||^2 (reduced deterministically) and
+ *     rho (s - z + u) s (1 - s) added into v_opacity [N].  rho is DEVICE float[1]; rho == 0 writes 0 and leaves
+ *     v_opacity alone.
+ *   Workspace: gsb_sparsity_workspace(N) bytes, 256-aligned.
+ *   gsb_adc_prune_classify: the final prune as a compaction for gsb_adc_apply.  Removes exactly n_prune rows: every
+ *     row with s below v, the n_prune-th smallest s, then the first rows in index order with s == v.  Writes counts
+ *     (DEVICE int32[8]) as gsb_adc_classify does -- [2] = n_prune, [3] = [4] = N - n_prune, the rest 0 -- and the
+ *     flags and ranks that gsb_adc_apply(N, src, dst, 0, N - n_prune, NULL, ...) reads.  Workspace:
+ *     gsb_adc_workspace(N) bytes, 256-aligned; N at most INT32_MAX / 2. */
+GSB_API size_t gsb_sparsity_workspace(uint32_t N);
+GSB_API int gsb_sparsity_update(uint32_t N, const float *opacity_raw, float *z, float *u, uint32_t k, int initialize,
+                                void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_sparsity_loss(uint32_t N, const float *opacity_raw, const float *z, const float *u,
+                              const float *rho /*DEVICE*/, float *v_opacity, float *loss_out /*DEVICE*/,
+                              void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_adc_prune_classify(uint32_t N, const float *opacity_raw, uint32_t n_prune,
+                                   int32_t *counts /*DEVICE [8]*/, void *workspace, size_t workspace_bytes,
+                                   gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

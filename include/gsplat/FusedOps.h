@@ -147,4 +147,18 @@ adc_apply(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &
 void adc_reset_opacity(at::Tensor opacity_raw, c10::optional<at::Tensor> exp_avg, c10::optional<at::Tensor> exp_avg_sq,
                        const float prune_opacity);
 
+// ADMM opacity sparsification (src/training/components/sparsity_optimizer.cpp).  k = (int)(prune_ratio * N), the
+// caller's float product.  Nothing is read back to the host.
+//
+// initialize (u = 0, z = prune_z(sigmoid(o))) or update_state (z = prune_z(sigmoid(o) + u), u += sigmoid(o) - z) in
+// place on z and u ([N] float, opacity_raw's element count)
+void sparsity_update(const at::Tensor opacity_raw, at::Tensor z, at::Tensor u, const int64_t k, const bool initialize);
+// 0.5 rho ||sigmoid(o) - z + u||^2 as a [1] device tensor; its gradient added into v_opacity.  rho: a [1] device
+// tensor (0: zero loss, v_opacity untouched)
+at::Tensor sparsity_loss(const at::Tensor opacity_raw, const at::Tensor z, const at::Tensor u, const at::Tensor rho,
+                         at::Tensor v_opacity);
+// the final prune: (counts [8], workspace) for adc_apply(..., n_split = 0, n_final = N - n_prune), which then removes
+// exactly the n_prune rows of lowest sigmoid(opacity_raw) (ties at the boundary: the first in index order)
+std::tuple<at::Tensor, at::Tensor> sparsity_prune_classify(const at::Tensor opacity_raw, const int64_t n_prune);
+
 } // namespace gsplat
