@@ -10,7 +10,10 @@
 //     matrix (148 KB in L2) instead of a third launch.  A pass whose digit is the same for every ACTIVE key
 //     (SortCtl::key_or / key_and, e.g. the exponent byte of depths within one octave) is skipped by both
 //     kernels; which buffer currently holds the data is derived from the same control block, so no host
-//     round trip is needed.
+//     round trip is needed.  Any subset of the passes may be skipped, all four included (one Gaussian with
+//     tiles, or all of them at one depth): the caller therefore writes the values (the identity permutation)
+//     into v0 together with the keys, so that whichever pass runs first -- or, when none does, the run
+//     table itself -- reads a valid permutation from v0.
 //   * scan_blocksum_kernel / scan_apply_kernel -- two-launch inclusive scan (per-CTA sums, then every CTA
 //     adds the sums of its predecessors and scans its own segment).
 // The kernels are stream-ordered and keep no state outside the caller's workspace.
@@ -83,19 +86,17 @@ __global__ void __launch_bounds__(kSortThreads) radix_count_kernel(const KeyT *_
 
 // ---- pass kernel 2: stable scatter ----------------------------------------------------------------------
 // Source / destination: without a control block k0/v0 -> k1/v1 (the host alternates the buffers); with one,
-// buffer (passes executed so far) & 1 is the source.  iota_first: the values of the first executed pass are
-// the element indices (v0 is not read).
+// buffer (passes executed so far) & 1 is the source.
 template <typename KeyT>
 __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(
     KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, uint32_t seg, uint32_t nblocks, int pass,
-    uint32_t shift, uint32_t mask, const SortCtl *__restrict__ ctl, const uint32_t *__restrict__ H, int iota_first) {
+    uint32_t shift, uint32_t mask, const SortCtl *__restrict__ ctl, const uint32_t *__restrict__ H) {
     if (radix_pass_skipped(ctl, pass)) return;
     const int done = ctl ? radix_passes_done(ctl, pass) : 0;
     const KeyT *__restrict__ ksrc = (done & 1) ? k1 : k0;
     KeyT *__restrict__ kdst = (done & 1) ? k0 : k1;
     const uint32_t *__restrict__ vsrc = (done & 1) ? v1 : v0;
     uint32_t *__restrict__ vdst = (done & 1) ? v0 : v1;
-    const bool iota = iota_first && done == 0;
 
     __shared__ uint32_t s_w[kSortWarps][kRadixBins]; // warp histograms, then warp write cursors
     __shared__ uint32_t s_tot[4][kRadixBins], s_pre[4][kRadixBins];
@@ -184,7 +185,7 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(
             const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
             const uint32_t pos = base + rank;
             kdst[pos] = key;
-            vdst[pos] = iota ? (uint32_t)i : vsrc[i];
+            vdst[pos] = vsrc[i];
             if ((peers >> lane) == 1u) cur[dgt] = base + __popc(peers); // highest lane of the group
         }
         __syncwarp();

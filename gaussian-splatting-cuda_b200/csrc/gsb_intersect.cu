@@ -102,7 +102,9 @@ __global__ void __launch_bounds__(kIsectThreads) isect_emit_kernel(uint64_t n, u
 
 // ---- planned path, step 1: tile box, count and depth key of every Gaussian ---------------------------------
 // boxes[idx] = (x0 | y0 << 16, w | h << 16) in tiles.  Gaussians without tiles get the key 0xffffffff: they
-// end up behind every Gaussian that has tiles and never enter the run table.
+// end up behind every Gaussian that has tiles and never enter the run table.  vals[idx] = idx is the depth
+// sort's initial permutation: the sort skips every pass whose digit is constant over the Gaussians with tiles,
+// possibly all four, so the first pass that runs -- or the run table, when none does -- reads it.
 __global__ void __launch_bounds__(kIsectThreads) isect_plan_kernel(uint64_t n, const float *__restrict__ means2d,
                                                                     const int32_t *__restrict__ radii,
                                                                     const float *__restrict__ depths,
@@ -110,6 +112,7 @@ __global__ void __launch_bounds__(kIsectThreads) isect_plan_kernel(uint64_t n, c
                                                                     uint32_t tile_height,
                                                                     int32_t *__restrict__ tiles_per_gauss,
                                                                     uint32_t *__restrict__ keys,
+                                                                    uint32_t *__restrict__ vals,
                                                                     uint2 *__restrict__ boxes,
                                                                     SortCtl *__restrict__ ctl) {
     __shared__ uint32_t s_or[kIsectThreads / 32], s_nor[kIsectThreads / 32];
@@ -127,6 +130,7 @@ __global__ void __launch_bounds__(kIsectThreads) isect_plan_kernel(uint64_t n, c
             k_nor = ~key;
         }
         keys[idx] = key;
+        vals[idx] = (uint32_t)idx;
         boxes[idx] = make_uint2(b.x0 | (b.y0 << 16), w | (h << 16));
     }
     k_or = __reduce_or_sync(0xffffffffu, k_or);
@@ -143,10 +147,12 @@ __global__ void __launch_bounds__(kIsectThreads) isect_plan_kernel(uint64_t n, c
 }
 
 // EWA path (SURVEY.md 8 f4): the front kernel of gsb_fastgs.cu has already computed every primitive's tile box and its
-// EXACT tile count; this step only derives the sort keys (depth bits, 0xffffffff for primitives without tiles).
+// EXACT tile count; this step only derives the sort keys (depth bits, 0xffffffff for primitives without tiles) and the
+// initial permutation.
 __global__ void __launch_bounds__(kIsectThreads) isect_plan_boxes_kernel(uint64_t n, const int32_t *__restrict__ counts,
                                                                           const float *__restrict__ depths,
                                                                           uint32_t *__restrict__ keys,
+                                                                          uint32_t *__restrict__ vals,
                                                                           SortCtl *__restrict__ ctl) {
     __shared__ uint32_t s_or[kIsectThreads / 32], s_nor[kIsectThreads / 32];
     const uint64_t idx = (uint64_t)blockIdx.x * kIsectThreads + threadIdx.x;
@@ -159,6 +165,7 @@ __global__ void __launch_bounds__(kIsectThreads) isect_plan_boxes_kernel(uint64_
             k_nor = ~key;
         }
         keys[idx] = key;
+        vals[idx] = (uint32_t)idx;
     }
     k_or = __reduce_or_sync(0xffffffffu, k_or);
     k_nor = __reduce_or_sync(0xffffffffu, k_nor);
@@ -737,8 +744,7 @@ static PlanWs plan_ws(uint64_t n, const BinPlan &b, const SegPlan &sp, bool filt
 
 template <typename KeyT>
 static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, const SegPlan &sp, int passes,
-                             uint32_t begin_bit, uint32_t end_bit, const SortCtl *ctl, uint32_t *H, bool iota_first,
-                             cudaStream_t s) {
+                             uint32_t begin_bit, uint32_t end_bit, const SortCtl *ctl, uint32_t *H, cudaStream_t s) {
     for (int pass = 0; pass < passes; ++pass) {
         const uint32_t shift = begin_bit + 8u * (uint32_t)pass;
         const uint32_t bits = end_bit - shift < 8u ? end_bit - shift : 8u;
@@ -749,7 +755,7 @@ static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uin
         radix_count_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, n, sp.seg, pass, shift, mask, ctl, H);
         GSB_LAUNCH_CHECK();
         radix_scatter_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, vs, vd, n, sp.seg, sp.nblocks, pass, shift,
-                                                                     mask, ctl, H, iota_first && pass == 0 ? 1 : 0);
+                                                                     mask, ctl, H);
         GSB_LAUNCH_CHECK();
     }
     return GSB_OK;
@@ -841,7 +847,7 @@ extern "C" int gsb_isect_sort(uint64_t n_isects, uint32_t C, uint32_t tile_width
     uint32_t *v0 = (passes & 1) ? tmp_v : out_v, *v1 = (passes & 1) ? out_v : tmp_v;
     GSB_CUDA_TRY(cudaMemcpyAsync(k0, isect_ids_in, n_isects * 8, cudaMemcpyDeviceToDevice, s));
     GSB_CUDA_TRY(cudaMemcpyAsync(v0, flatten_ids_in, n_isects * 4, cudaMemcpyDeviceToDevice, s));
-    return radix_sort_launch<unsigned long long>(k0, k1, v0, v1, n_isects, sp, passes, 0, end_bit, nullptr, H, false, s);
+    return radix_sort_launch<unsigned long long>(k0, k1, v0, v1, n_isects, sp, passes, 0, end_bit, nullptr, H, s);
 }
 
 extern "C" size_t gsb_isect_plan_workspace(uint32_t C, uint32_t N, uint32_t tile_width, uint32_t tile_height) {
@@ -905,15 +911,15 @@ static int plan_impl(uint32_t C, uint32_t N, const PlanSource &src, const float 
         GSB_CUDA_TRY(cudaMemsetAsync(ctl, 0, sizeof(SortCtl), s));
         const uint32_t grid = (uint32_t)((n + kIsectThreads - 1) / kIsectThreads);
         if (src.ewa())
-            isect_plan_boxes_kernel<<<grid, kIsectThreads, 0, s>>>(n, tiles_per_gauss, depths, k0, ctl);
+            isect_plan_boxes_kernel<<<grid, kIsectThreads, 0, s>>>(n, tiles_per_gauss, depths, k0, v0, ctl);
         else
             isect_plan_kernel<<<grid, kIsectThreads, 0, s>>>(n, src.means2d, src.radii, depths, src.tile_size, tile_width,
-                                                            tile_height, tiles_per_gauss, k0, boxes, ctl);
+                                                            tile_height, tiles_per_gauss, k0, v0, boxes, ctl);
         GSB_LAUNCH_CHECK();
     }
     {
         ProfScope ps("isect_depth_sort", s);
-        if (int rc = radix_sort_launch<uint32_t>(k0, k1, v0, v1, n, sp, 4, 0, 32, ctl, H, true, s)) return rc;
+        if (int rc = radix_sort_launch<uint32_t>(k0, k1, v0, v1, n, sp, 4, 0, 32, ctl, H, s)) return rc;
     }
     {
         ProfScope ps("isect_runs", s);

@@ -91,6 +91,37 @@ def scene_small(N=2000, width=200, height=120, sh_degree=3, seed=7, view=None):
     return _finish(rng, N, sh_degree, means, scales, width, height, 160.0, 170.0, viewmat=viewmat)
 
 
+def scene_one_visible(N=2000, width=200, height=120, sh_degree=3, seed=13):
+    """One Gaussian in view, every other one culled: behind the camera, or far outside the frustum.  With a single
+    Gaussian that has tiles, the intersect stage's depth sort skips all four of its radix passes."""
+    rng = np.random.default_rng(seed)
+    means = np.empty((N, 3), np.float32)
+    means[:, 0] = rng.random(N, dtype=np.float32) * 3.0 - 1.5
+    means[:, 1] = rng.random(N, dtype=np.float32) * 1.8 - 0.9
+    means[:, 2] = -(rng.random(N, dtype=np.float32) * 2.0 + 1.0)  # behind the camera
+    side = rng.random(N) < 0.3
+    means[side, 0] = np.where(rng.random(int(side.sum())) < 0.5, -60.0, 60.0)  # in front, 20x the frustum's width away
+    means[side, 2] = rng.random(int(side.sum()), dtype=np.float32) * 2.0 + 2.0
+    k = N // 2
+    means[k] = (0.05, -0.03, 2.5)
+    scales = np.exp(rng.random((N, 3), dtype=np.float32) * (np.log(0.15) - np.log(0.02)) + np.log(0.02))
+    scales[k] = (0.4, 0.25, 0.3)  # covers most of the frame
+    return _finish(rng, N, sh_degree, means, scales, width, height, 160.0, 170.0)
+
+
+def scene_wall(N=1500, width=200, height=120, sh_degree=3, seed=17, depth=3.0):
+    """A fronto-parallel wall: identity view and every Gaussian at camera depth `depth` exactly, with footprints large
+    enough to overlap many times, so the order of equal-depth Gaussians (ascending index, the reference's stable sort)
+    decides the image.  The intersect stage's depth sort skips all four of its radix passes."""
+    rng = np.random.default_rng(seed)
+    means = np.empty((N, 3), np.float32)
+    means[:, 0] = rng.random(N, dtype=np.float32) * 4.4 - 2.2
+    means[:, 1] = rng.random(N, dtype=np.float32) * 2.6 - 1.3
+    means[:, 2] = depth
+    scales = np.exp(rng.random((N, 3), dtype=np.float32) * (np.log(0.12) - np.log(0.04)) + np.log(0.04))
+    return _finish(rng, N, sh_degree, means, scales, width, height, 160.0, 170.0)
+
+
 def fastgs_inputs(scene: dict, seed: int = 3) -> dict:
     """The RAW parameters the reference's fastgs rasterizer takes (fast_rasterizer.cpp:24-54) for a scene dict:
     log-scales, un-normalised quaternions, logit opacities, sh0 / shN split, w2c and the camera position."""

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import scenes
+from isect_fixtures import WINDOW_TILES
 
 pytestmark = pytest.mark.gpu
 
@@ -20,7 +21,12 @@ def _project(native, sc, dev):
     return radii, means2d, depths
 
 
-@pytest.mark.parametrize("n_gauss,views,scale_mul", [(200_000, (1,), 1.0), (50_000, (1,), 4.0), (100_000, (1, 3), 2.0)])
+# five 1080p cameras: 40 800 (camera, tile) pairs, more than one window of the histogram and placement
+WINDOWED_VIEWS = (0, 1, 2, 3, 5)
+
+
+@pytest.mark.parametrize("n_gauss,views,scale_mul", [(200_000, (1,), 1.0), (50_000, (1,), 4.0), (100_000, (1, 3), 2.0),
+                                                     (50_000, WINDOWED_VIEWS, 2.0)])
 def test_diagonal_view_lists_equal_oracle(native, orc, cuda_device, n_gauss, views, scale_mul):
     per_view = [_project(native, scenes.scene_b(N=n_gauss, view=v, scale_mul=scale_mul), cuda_device) for v in views]
     radii, means2d, depths = (torch.cat([pv[i] for pv in per_view], 0).contiguous() for i in range(3))
@@ -35,10 +41,15 @@ def test_diagonal_view_lists_equal_oracle(native, orc, cuda_device, n_gauss, vie
     # the scene exercises what the placement has to keep in order
     tiles = (ids_ref >> 32).astype(np.int64)
     n = tpg_ref.reshape(-1)
+    glob = (tiles >> (tw * th).bit_length()) * (tw * th) + (tiles & ((1 << (tw * th).bit_length()) - 1))
+    windows = -(-C * tw * th // WINDOW_TILES)
     print(f"views {views} x{scale_mul}: {len(ids_ref)} intersections, largest tile list {np.bincount(tiles).max()}, "
-          f"largest box {n.max()} tiles")
+          f"largest box {n.max()} tiles, {C * tw * th} tiles in {windows} windows "
+          f"({int((glob >= WINDOW_TILES).sum())} intersections past the first)")
     if scale_mul > 1.0:
         assert n.max() > 32
+    if views == WINDOWED_VIEWS:
+        assert C * tw * th > WINDOW_TILES and (glob >= WINDOW_TILES).sum() > 1000
     assert np.array_equal(tpg.cpu().numpy(), tpg_ref)
     assert np.array_equal(off.cpu().numpy(), off_ref)
     assert np.array_equal(ids.cpu().numpy(), ids_ref)
@@ -49,9 +60,25 @@ def test_diagonal_view_ewa_instances_in_order(native, cuda_device):
     """The fastgs (EWA) path places with the per-tile ellipse test: every tile's instances must be ordered by (depth bits,
     index), and every primitive must sit in exactly the tiles of its box that pass the test -- the front kernel's mask
     for boxes of up to 32 tiles, as many tiles as its exact count for the larger ones (those re-evaluate the test)."""
+    _check_ewa_instances(native, cuda_device, scenes.scene_b(N=50_000, view=1, scale_mul=4.0))
+
+
+def test_windowed_ewa_instances_in_order(native, cuda_device):
+    """The same at 4112x2320: 37 265 tiles, two windows of the histogram and placement.  The longer focal length
+    spreads the slab over the whole frame, so the second window (the last tile row) receives instances too."""
+    sc = scenes.scene_b(N=50_000, width=4112, height=2320, view=1, scale_mul=2.0)
+    sc["Ks"][0, 0, 0] = sc["Ks"][0, 1, 1] = 2400.0
+    tile = _check_ewa_instances(native, cuda_device, sc)
+    n_tiles = ((4112 + 15) // 16) * ((2320 + 15) // 16)
+    past = int((tile >= WINDOW_TILES).sum())
+    print(f"{n_tiles} tiles in {-(-n_tiles // WINDOW_TILES)} windows, {past} instances past the first")
+    assert n_tiles > WINDOW_TILES and past > 100
+
+
+def _check_ewa_instances(native, cuda_device, scene):
     import importlib
     fg = importlib.import_module(native.__name__ + ".fastgs")
-    inp = scenes.fastgs_inputs(scenes.scene_b(N=50_000, view=1, scale_mul=4.0))
+    inp = scenes.fastgs_inputs(scene)
     P = {k: torch.from_numpy(inp[k]).to(cuda_device) for k in
          ("means", "scales_raw", "rotations_raw", "opacities_raw", "sh0", "shN")}
     s = fg.FastGSSettings(cam_position=torch.from_numpy(inp["cam_position"]).to(cuda_device),
@@ -97,3 +124,4 @@ def test_diagonal_view_ewa_instances_in_order(native, cuda_device):
     print(f"{len(inst)} instances, largest box {int((w * h).max())} tiles, {int((~small).sum())} instances of boxes "
           f"larger than 32 tiles, largest tile list {int(np.diff(toff).max())}")
     assert (~small).sum() > 0
+    return tile

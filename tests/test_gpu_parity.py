@@ -155,6 +155,10 @@ def _blend_case(name):
         return scenes.scene_small(N=3000, width=200, height=120, view=1)
     if name == "b30k":
         return scenes.scene_b(N=30000, width=640, height=360, view=3, scale_mul=2.0)
+    if name == "one_visible":  # the intersect stage's depth sort skips all four passes (tests/isect_fixtures.py)
+        return scenes.scene_one_visible()
+    if name == "wall":  # the same, and every tile's order is decided by the ties of equal depths
+        return scenes.scene_wall()
     raise KeyError(name)
 
 
@@ -264,7 +268,7 @@ def test_blend_empty_inputs(native, cuda_device):
 # ------------------------------------------------------------------------------------------
 # whole path through the L3 mirror (autograd), against the oracle pipeline
 # ------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", ["small_rot", "a", "b30k"])
+@pytest.mark.parametrize("name", ["small_rot", "a", "b30k", "one_visible", "wall"])
 def test_pipeline_autograd_vs_oracle(native, orc, cuda_device, name):
     """Whole L3 path (SH -> intersect -> blend and the autograd chain back to every parameter) against the oracle
     pipeline.  Both sides are given the SAME projection outputs (the oracle's): a radius that flips at a ceil()
