@@ -21,8 +21,7 @@ from dataclasses import dataclass
 import torch
 
 from . import _product_ns, load
-
-PARAM_GROUPS = ("means", "sh0", "shN", "scaling_raw", "rotation_raw", "opacity_raw")
+from .strategy import PARAM_GROUPS, Strategy
 
 
 def lowest_opacity_removed(params: list, exp_avg: list, exp_avg_sq: list, n_prune: int):
@@ -62,7 +61,7 @@ class DefaultConfig:
     max_cap: int = 1000000
 
 
-class DefaultStrategy:
+class DefaultStrategy(Strategy):
     """The strategy over a parameter dict (PARAM_GROUPS -> leaf tensors) and its FusedAdam.  Mutates both: after a
     refine that changed the set, params[k] and optimizer.exp_avg[k] / exp_avg_sq[k] are new tensors.  scene_scale is
     the optimizer's (one get_scene_scale() feeds both the means learning rate and the thresholds)."""
@@ -76,7 +75,6 @@ class DefaultStrategy:
         dev = params["means"].device
         # strategy_utils.cpp:17 (initialize_gaussians): [2, N] zeros; the fastgs backward accumulates into it
         self.densification_info = torch.zeros((2, self.n), dtype=torch.float32, device=dev)
-        self.replaced = False    # the last refine replaced the tensors
         self.last_counts = None  # (duplicated, split, pruned, final rows) of the last refine
         self.last_z = None       # the last split's normals [2, n_split, 3]
         self.last_kept_split = 0
@@ -106,7 +104,7 @@ class DefaultStrategy:
 
     def grow_and_prune(self, iteration: int) -> bool:
         """grow_gs then prune_gs (default_strategy.cpp:164-249).  True when the set changed (the tensors are new)."""
-        ns, c, P, opt = _product_ns(), self.cfg, self.params, self.optimizer
+        ns, c, P = _product_ns(), self.cfg, self.params
         info = self.densification_info
         with torch.no_grad():
             counts, ws = ns.adc_classify(info if info.numel() else None, P["scaling_raw"].detach(),
@@ -126,25 +124,29 @@ class DefaultStrategy:
             if n_split > 0:  # default_strategy.cpp:100-104: the same call and shape, drawn only when rows split
                 z = torch.randn((2, n_split, 3), device=P["means"].device)
             self.last_z = z
-            out_p, out_m1, out_m2, new_info = ns.adc_apply(
-                [P[k].detach() for k in PARAM_GROUPS], [opt.exp_avg[k] for k in PARAM_GROUPS],
-                [opt.exp_avg_sq[k] for k in PARAM_GROUPS], ws, counts, n_split, n_final, z, bool(c.revised_opacity))
-        for k, p, m1, m2 in zip(PARAM_GROUPS, out_p, out_m1, out_m2):
-            P[k] = p.requires_grad_(True)
-            opt.exp_avg[k], opt.exp_avg_sq[k] = m1, m2
+            out_p, out_m1, out_m2, new_info = ns.adc_apply(*self._state(), ws, counts, n_split, n_final, z,
+                                                           bool(c.revised_opacity))
+        self._install(out_p, out_m1, out_m2)
         self.densification_info = new_info
         return True
+
+    def _state(self):
+        """(params, exp_avg, exp_avg_sq) as lists in PARAM_GROUPS order."""
+        P, opt = self.params, self.optimizer
+        return ([P[k].detach() for k in PARAM_GROUPS], [opt.exp_avg[k] for k in PARAM_GROUPS],
+                [opt.exp_avg_sq[k] for k in PARAM_GROUPS])
+
+    def _install(self, params: list, exp_avg: list, exp_avg_sq: list) -> None:
+        """New tensors become the leaves and their moments the optimizer's; step counts are kept."""
+        for k, p, m1, m2 in zip(PARAM_GROUPS, params, exp_avg, exp_avg_sq):
+            self.params[k] = p.requires_grad_(True)
+            self.optimizer.exp_avg[k], self.optimizer.exp_avg_sq[k] = m1, m2
 
     def remove_lowest_opacity(self, n_prune: int) -> None:
         """remove_gaussians (default_strategy.cpp:194-227) of the n_prune lowest-opacity rows: new tensors and
         moments, step counts kept.  Non-empty statistics become zeros [2, n_kept]."""
-        P, opt = self.params, self.optimizer
-        out_p, out_m1, out_m2, new_info = lowest_opacity_removed(
-            [P[k].detach() for k in PARAM_GROUPS], [opt.exp_avg[k] for k in PARAM_GROUPS],
-            [opt.exp_avg_sq[k] for k in PARAM_GROUPS], n_prune)
-        for k, p, m1, m2 in zip(PARAM_GROUPS, out_p, out_m1, out_m2):
-            P[k] = p.requires_grad_(True)
-            opt.exp_avg[k], opt.exp_avg_sq[k] = m1, m2
+        out_p, out_m1, out_m2, new_info = lowest_opacity_removed(*self._state(), n_prune)
+        self._install(out_p, out_m1, out_m2)
         if self.densification_info.numel():
             self.densification_info = new_info
 
@@ -178,12 +180,4 @@ class DefaultStrategy:
             self.reset_opacity()
             if not skip:
                 skip = ("opacity_raw",)
-        return skip
-
-    def post_backward(self, iteration: int) -> tuple:
-        """default_strategy.cpp:292-326.  The skipped groups lose their gradient, so that the following FusedAdam step
-        leaves them and their step counts alone."""
-        skip = self.refine(iteration)
-        for k in skip:
-            self.params[k].grad = None
         return skip

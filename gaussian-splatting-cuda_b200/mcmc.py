@@ -2,8 +2,8 @@
 this library's kernels (csrc/gsb_mcmc.cu).
 
   post_backward(iteration)   mcmc.cpp:369-393: SH-degree bump, then -- on a refine iteration -- relocate_gs and
-                             add_new_gs, then inject_noise with lr(group 0) * 5e5 (the rate before this iteration's
-                             scheduler step)
+                             add_new_gs, then inject_noise (before_adam) with lr(group 0) * 5e5 (the rate before this
+                             iteration's scheduler step)
   regularize(params)         trainer.cpp:132-158: scale_reg * mean(exp(scaling_raw)) + opacity_reg *
                              mean(sigmoid(opacity_raw)), gradients added into the parameters' .grad
 
@@ -26,8 +26,7 @@ import numpy as np
 import torch
 
 from . import _product_ns, load
-
-PARAM_GROUPS = ("means", "sh0", "shN", "scaling_raw", "rotation_raw", "opacity_raw")
+from .strategy import PARAM_GROUPS, Strategy
 
 
 @dataclass
@@ -64,7 +63,7 @@ def growth_count(n: int, max_cap: int) -> int:
     return max(0, target - n)
 
 
-class MCMC:
+class MCMC(Strategy):
     """The strategy over a parameter dict (PARAM_GROUPS -> leaf tensors) and its FusedAdam.  Mutates both in place:
     after a growth step params[k] and optimizer.exp_avg[k] / exp_avg_sq[k] are new [:N] views of the storage."""
 
@@ -170,19 +169,18 @@ class MCMC:
                                              c.opacity_reg, gs if c.scale_reg > 0 else None,
                                              go if c.opacity_reg > 0 else None)
 
-    def refine(self, iteration: int) -> bool:
-        """The SH bump and, on a refine iteration, relocation then growth.  True when rows were added."""
+    def before_adam(self, lr: float | torch.Tensor) -> None:
+        self.inject_noise(lr)
+
+    def refine(self, iteration: int) -> tuple:
+        """The SH bump and, on a refine iteration, relocation then growth.  A growth replaces the tensors, so Adam
+        skips every group (nothing to step, as after the reference's torch::cat); relocation works in place."""
         if iteration % self.cfg.sh_degree_interval == 0 and self.sh_degree < self.cfg.sh_degree:
             self.sh_degree += 1
+        self.replaced = False
         if not self.is_refining(iteration):
-            return False
+            return ()
         self.refines += 1
         self.relocate()
-        return self.grow() > 0
-
-    def post_backward(self, iteration: int, lr: float | torch.Tensor | None = None) -> bool:
-        """mcmc.cpp:369-393.  lr defaults to the optimizer's group-0 rate.  True when rows were added (the following
-        Adam step then has nothing to step)."""
-        grew = self.refine(iteration)
-        self.inject_noise(self.optimizer.lr[0] if lr is None else lr)
-        return grew
+        self.replaced = self.grow() > 0
+        return PARAM_GROUPS if self.replaced else ()

@@ -251,17 +251,17 @@ GSB_EXPORT std::tuple<at::Tensor, at::Tensor> photometric_loss_fused_unclamped(c
     return photometric_loss_impl(renders, target, lambda_dssim, compute_grad, GSB_LOSS_NO_CLAMP);
 }
 
-GSB_EXPORT void fused_adam_step(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,
-                                const std::vector<at::Tensor> &exp_avg, const std::vector<at::Tensor> &exp_avg_sq,
-                                const std::vector<double> &lr, const double beta1, const double beta2, const double eps,
-                                const std::vector<int64_t> &step_counts) {
+namespace {
+// Validates one entry per group in every list and packs the groups' tensors and hyperparameters into g; the learning
+// rate and the bias corrections are the caller's.  Returns the number of groups.
+uint32_t pack_adam_groups(const char *op, GsbAdamGroup (&g)[8], const std::vector<at::Tensor> &params,
+                          const std::vector<at::Tensor> &grads, const std::vector<at::Tensor> &exp_avg,
+                          const std::vector<at::Tensor> &exp_avg_sq, const double beta1, const double beta2,
+                          const double eps) {
     const size_t n = params.size();
-    TORCH_CHECK(n > 0 && n <= 8, "fused_adam_step: 1..8 parameter groups");
-    TORCH_CHECK(grads.size() == n && exp_avg.size() == n && exp_avg_sq.size() == n && lr.size() == n &&
-                    step_counts.size() == n,
-                "fused_adam_step: one entry per group in every list");
-    const c10::cuda::CUDAGuard guard(params[0].device());
-    GsbAdamGroup g[8];
+    TORCH_CHECK(n > 0 && n <= 8, op, ": 1..8 parameter groups");
+    TORCH_CHECK(grads.size() == n && exp_avg.size() == n && exp_avg_sq.size() == n, op,
+                ": one entry per group in every list");
     for (size_t i = 0; i < n; ++i) {
         CHECK_F32(params[i]);
         CHECK_F32(grads[i]);
@@ -269,42 +269,7 @@ GSB_EXPORT void fused_adam_step(const std::vector<at::Tensor> &params, const std
         CHECK_F32(exp_avg_sq[i]);
         TORCH_CHECK(grads[i].numel() == params[i].numel() && exp_avg[i].numel() == params[i].numel() &&
                         exp_avg_sq[i].numel() == params[i].numel(),
-                    "fused_adam_step: group ", i, " has mismatching sizes");
-        g[i].param = params[i].data_ptr<float>();
-        g[i].grad = grads[i].data_ptr<float>();
-        g[i].exp_avg = exp_avg[i].data_ptr<float>();
-        g[i].exp_avg_sq = exp_avg_sq[i].data_ptr<float>();
-        g[i].n = (uint64_t)params[i].numel();
-        g[i].lr = (float)lr[i];
-        g[i].beta1 = (float)beta1;
-        g[i].beta2 = (float)beta2;
-        g[i].eps = (float)eps;
-        // fused_adam.cpp:80-81
-        g[i].bias_correction1_rcp = (float)(1.0 / (1.0 - std::pow(beta1, (double)step_counts[i])));
-        g[i].bias_correction2_sqrt_rcp = (float)(1.0 / std::sqrt(1.0 - std::pow(beta2, (double)step_counts[i])));
-    }
-    gsb_check(gsb_adam_step(g, (uint32_t)n, cur_stream()), "fused_adam_step");
-}
-
-GSB_EXPORT void fused_adam_step_dynamic(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,
-                                        const std::vector<at::Tensor> &exp_avg, const std::vector<at::Tensor> &exp_avg_sq,
-                                        const at::Tensor dynamic_scalars, const double beta1, const double beta2,
-                                        const double eps) {
-    const size_t n = params.size();
-    TORCH_CHECK(n > 0 && n <= 8, "fused_adam_step_dynamic: 1..8 parameter groups");
-    TORCH_CHECK(grads.size() == n && exp_avg.size() == n && exp_avg_sq.size() == n, "one entry per group in every list");
-    CHECK_F32(dynamic_scalars);
-    TORCH_CHECK(dynamic_scalars.numel() == (int64_t)n * 4, "dynamic_scalars must be [n_groups, 4]");
-    const c10::cuda::CUDAGuard guard(params[0].device());
-    GsbAdamGroup g[8];
-    for (size_t i = 0; i < n; ++i) {
-        CHECK_F32(params[i]);
-        CHECK_F32(grads[i]);
-        CHECK_F32(exp_avg[i]);
-        CHECK_F32(exp_avg_sq[i]);
-        TORCH_CHECK(grads[i].numel() == params[i].numel() && exp_avg[i].numel() == params[i].numel() &&
-                        exp_avg_sq[i].numel() == params[i].numel(),
-                    "fused_adam_step_dynamic: group ", i, " has mismatching sizes");
+                    op, ": group ", i, " has mismatching sizes");
         g[i].param = params[i].data_ptr<float>();
         g[i].grad = grads[i].data_ptr<float>();
         g[i].exp_avg = exp_avg[i].data_ptr<float>();
@@ -316,8 +281,39 @@ GSB_EXPORT void fused_adam_step_dynamic(const std::vector<at::Tensor> &params, c
         g[i].eps = (float)eps;
         g[i].bias_correction1_rcp = g[i].bias_correction2_sqrt_rcp = 1.f;
     }
-    gsb_check(gsb_adam_step_dynamic(g, (uint32_t)n, dynamic_scalars.data_ptr<float>(), cur_stream()),
-              "fused_adam_step_dynamic");
+    return (uint32_t)n;
+}
+} // namespace
+
+GSB_EXPORT void fused_adam_step(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,
+                                const std::vector<at::Tensor> &exp_avg, const std::vector<at::Tensor> &exp_avg_sq,
+                                const std::vector<double> &lr, const double beta1, const double beta2, const double eps,
+                                const std::vector<int64_t> &step_counts) {
+    TORCH_CHECK(lr.size() == params.size() && step_counts.size() == params.size(),
+                "fused_adam_step: one entry per group in every list");
+    GsbAdamGroup g[8];
+    const uint32_t n = pack_adam_groups("fused_adam_step", g, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps);
+    const c10::cuda::CUDAGuard guard(params[0].device());
+    for (uint32_t i = 0; i < n; ++i) {
+        g[i].lr = (float)lr[i];
+        // fused_adam.cpp:80-81
+        g[i].bias_correction1_rcp = (float)(1.0 / (1.0 - std::pow(beta1, (double)step_counts[i])));
+        g[i].bias_correction2_sqrt_rcp = (float)(1.0 / std::sqrt(1.0 - std::pow(beta2, (double)step_counts[i])));
+    }
+    gsb_check(gsb_adam_step(g, n, cur_stream()), "fused_adam_step");
+}
+
+GSB_EXPORT void fused_adam_step_dynamic(const std::vector<at::Tensor> &params, const std::vector<at::Tensor> &grads,
+                                        const std::vector<at::Tensor> &exp_avg, const std::vector<at::Tensor> &exp_avg_sq,
+                                        const at::Tensor dynamic_scalars, const double beta1, const double beta2,
+                                        const double eps) {
+    GsbAdamGroup g[8];
+    const uint32_t n =
+        pack_adam_groups("fused_adam_step_dynamic", g, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps);
+    CHECK_F32(dynamic_scalars);
+    TORCH_CHECK(dynamic_scalars.numel() == (int64_t)n * 4, "dynamic_scalars must be [n_groups, 4]");
+    const c10::cuda::CUDAGuard guard(params[0].device());
+    gsb_check(gsb_adam_step_dynamic(g, n, dynamic_scalars.data_ptr<float>(), cur_stream()), "fused_adam_step_dynamic");
 }
 
 } // namespace gsplat

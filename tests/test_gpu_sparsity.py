@@ -319,7 +319,8 @@ def test_refine_at_the_base_iteration_raises(native, cuda_device):
 @pytest.mark.parametrize("path", ["gsplat", "fastgs"])
 def test_graphed_equals_eager(native, cuda_device, path, kind):
     """The graphed step against the eager one from the same seeds, base 20, 120 steps, and two iterations after the
-    prune.  Captures: the first, one at phase entry (20) and one after the prune (141) -- no others."""
+    prune.  Captures: the first, one at phase entry (20) and one after the prune (141) -- no others.  After the base
+    iteration neither step runs post_backward, so MCMC injects no noise: not in the re-capture at 141 either."""
     sp_mod = _mods(native)[0]
     prob, raw = _problem(native, path, cuda_device)
     runs = []
@@ -330,6 +331,8 @@ def test_graphed_equals_eager(native, cuda_device, path, kind):
         runs.append((strat, Q, step, run, [], []))
     _, _, g, _, _, captures_at = runs[1]
     for it in range(1, 143):
+        if it == 141 and kind == "mcmc":
+            noise = [r[0].last_noise for r in runs]
         for strat, Q, step, run, losses, caps in runs:
             torch.manual_seed(1000 + it)
             c = getattr(step, "captures", 0)
@@ -339,6 +342,8 @@ def test_graphed_equals_eager(native, cuda_device, path, kind):
     (sa, A, _, _, la, _), (sb, B, _, _, lb, _), (sc, C, _, _, lc, _) = runs
     print(path, kind, "captures at", captures_at, "N", sa.n)
     assert captures_at == [1, 20, 141] and g.captures == 3
+    if kind == "mcmc":
+        assert all(n is not None and r[0].last_noise is n for r, n in zip(runs, noise))
     assert sa.n == sb.n == sc.n == 3000 - R.prune_index(0.6, 3000) if path == "fastgs" else sa.n == sb.n
     for a, b, c in zip(la, lb, lc):
         assert abs(a - b) <= max(1e-3 * max(1.0, abs(a)), 5 * abs(a - c))
