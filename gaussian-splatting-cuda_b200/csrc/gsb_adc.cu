@@ -7,7 +7,7 @@
 //   gsb_adc_classify  per row: dup = high & small, split = high & !small, whether the row (and its duplicate copy)
 //                     survives the prune, whether its split copies do (read from the copies' stored scaling_raw and,
 //                     with revised_opacity, their stored opacity, computed as torch computes them); then one scan of
-//                     four counters over those flags (gsb_devsort.cuh's scan kernels with a Cnt4 accumulator):
+//                     four counters over those flags (gsb_scan.cuh's scan kernels with a Cnt4 accumulator):
 //                     rank among split rows (indexes z), among kept rest rows, kept duplicate copies and kept split
 //                     rows.  The totals go to a small DEVICE array: the one value a refine reads back.
 //   gsb_adc_apply     the final row of every output is a segment base plus a rank, in the reference's order
@@ -25,7 +25,7 @@
 #include <cmath>
 
 #include "gsb_common.cuh"
-#include "gsb_devsort.cuh"
+#include "gsb_scan.cuh"
 #include "gsb_select.cuh"
 
 namespace gsb {
@@ -50,16 +50,16 @@ struct Cnt4 {
         return *this;
     }
     __device__ __forceinline__ Cnt4 operator+(const Cnt4 &o) const { Cnt4 r = *this; return r += o; }
+    // found by argument-dependent lookup from block_scan_inclusive
+    friend __device__ __forceinline__ Cnt4 __shfl_up_sync(unsigned mask, const Cnt4 &v, int delta) {
+        Cnt4 r;
+        r.split = ::__shfl_up_sync(mask, v.split, delta);
+        r.rest = ::__shfl_up_sync(mask, v.rest, delta);
+        r.dup = ::__shfl_up_sync(mask, v.dup, delta);
+        r.spl = ::__shfl_up_sync(mask, v.spl, delta);
+        return r;
+    }
 };
-// found by argument-dependent lookup from block_scan_inclusive
-__device__ __forceinline__ Cnt4 __shfl_up_sync(unsigned mask, const Cnt4 &v, int delta) {
-    Cnt4 r;
-    r.split = ::__shfl_up_sync(mask, v.split, delta);
-    r.rest = ::__shfl_up_sync(mask, v.rest, delta);
-    r.dup = ::__shfl_up_sync(mask, v.dup, delta);
-    r.spl = ::__shfl_up_sync(mask, v.spl, delta);
-    return r;
-}
 
 struct LoadFlags {
     const uint8_t *f;
@@ -75,28 +75,24 @@ struct LoadFlags {
 };
 
 struct Ws {
-    Cnt4 *bsum;     // [kScanBlocks]
-    uint8_t *flags; // [N]
-    Cnt4 *ranks;    // [N] inclusive
-    uint32_t *map;  // [2N] output row -> source | kind
+    sel::SelectState *st; // the final prune's select
+    uint32_t *hist;        // [sel::kHistBytes / 4] its histograms
+    Cnt4 *bsum;            // [kScanBlocks]
+    uint8_t *flags;        // [N]
+    Cnt4 *ranks;           // [N] inclusive
+    uint32_t *map;         // [2N] output row -> source | kind; the final prune's keys in its first N entries
 };
 
-static size_t ws_bytes(uint32_t N) {
-    return 256 + (size_t)kScanBlocks * sizeof(Cnt4) + (((size_t)N + 15) & ~(size_t)15) + (size_t)N * sizeof(Cnt4) +
-           (size_t)N * 2 * sizeof(uint32_t);
-}
-
-static int ws_carve(uint32_t N, void *workspace, size_t bytes, Ws &w) {
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || bytes < ws_bytes(N)) return GSB_E_WORKSPACE;
-    char *b = static_cast<char *>(workspace) + 256;
-    w.bsum = reinterpret_cast<Cnt4 *>(b);
-    b += (size_t)kScanBlocks * sizeof(Cnt4);
-    w.flags = reinterpret_cast<uint8_t *>(b);
-    b += ((size_t)N + 15) & ~(size_t)15;
-    w.ranks = reinterpret_cast<Cnt4 *>(b);
-    b += (size_t)N * sizeof(Cnt4);
-    w.map = reinterpret_cast<uint32_t *>(b);
-    return GSB_OK;
+// the buffers of a workspace at `base` (null: sizing only); returns its size
+static size_t ws_layout(uint32_t N, void *base, Ws &w) {
+    WsLayout l{static_cast<char *>(base)};
+    w.st = l.carve<sel::SelectState>(1);
+    w.hist = l.carve<uint32_t>(sel::kHistBytes / sizeof(uint32_t));
+    w.bsum = l.carve<Cnt4>(kScanBlocks);
+    w.flags = l.carve<uint8_t>(N);
+    w.ranks = l.carve<Cnt4>(N);
+    w.map = l.carve<uint32_t>((size_t)N * 2);
+    return l.bytes;
 }
 
 struct Thresholds {
@@ -292,10 +288,7 @@ __global__ void __launch_bounds__(kThreads) reset_opacity_kernel(uint32_t N, flo
 }
 
 // ---- the sparsifier's final prune (gsb_adc_prune_classify) --------------------------------------------------------
-// Workspace reuse: the keys live in `map` (written by gsb_adc_apply only), the select's histograms in `bsum` (before
-// the scan uses it), its state in the 256-byte head.
-static_assert(sel::kHistBytes <= kScanBlocks * sizeof(Cnt4), "the select histograms must fit the scan's block sums");
-static_assert(sizeof(sel::SelectState) <= 256, "the select state must fit the workspace head");
+// The keys live in `map`, which only gsb_adc_apply writes.
 
 __global__ void __launch_bounds__(kThreads) prune_keys_kernel(uint32_t N, const float *__restrict__ opacity_raw,
                                                               uint32_t *__restrict__ keys) {
@@ -339,8 +332,6 @@ __global__ void __launch_bounds__(kThreads) prune_ranks_kernel(uint32_t N, uint3
     ranks[i] = r;
 }
 
-static unsigned blocks_for(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
-
 static bool rows_valid(const GsbMcmcRows &r) {
     if (!r.means || !r.sh0 || !r.scaling_raw || !r.rotation_raw || !r.opacity_raw || (r.shN_rows && !r.shN)) return false;
     return (reinterpret_cast<uintptr_t>(r.rotation_raw) & 15) == 0;
@@ -349,7 +340,10 @@ static bool rows_valid(const GsbMcmcRows &r) {
 } // namespace adc
 } // namespace gsb
 
-extern "C" size_t gsb_adc_workspace(uint32_t N) { return gsb::adc::ws_bytes(N); }
+extern "C" size_t gsb_adc_workspace(uint32_t N) {
+    gsb::adc::Ws w;
+    return gsb::adc::ws_layout(N, nullptr, w);
+}
 
 extern "C" int gsb_adc_classify(uint32_t N, const float *densification_info, const float *scaling_raw,
                                 const float *rotation_raw, const float *opacity_raw, const GsbAdcParams *params,
@@ -366,22 +360,15 @@ extern "C" int gsb_adc_classify(uint32_t N, const float *densification_info, con
     if (!scaling_raw || !rotation_raw || !opacity_raw) return GSB_E_INVALID;
     if (reinterpret_cast<uintptr_t>(rotation_raw) & 15) return GSB_E_INVALID;
     Ws w;
-    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, ws_layout(N, workspace, w))) return rc;
     const Thresholds t = thresholds(*params);
     ProfScope ps("adc_classify", s);
     GSB_CUDA_TRY(cudaMemsetAsync(counts, 0, 8 * sizeof(int32_t), s));
-    classify_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, densification_info, scaling_raw,
-                                                       reinterpret_cast<const float4 *>(rotation_raw), opacity_raw, t,
-                                                       w.flags, counts);
+    classify_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, densification_info, scaling_raw,
+                                                               reinterpret_cast<const float4 *>(rotation_raw),
+                                                               opacity_raw, t, w.flags, counts);
     GSB_LAUNCH_CHECK();
-    uint64_t nb = (N + 4095) / 4096;
-    if (nb > kScanBlocks) nb = kScanBlocks;
-    const uint32_t seg = (uint32_t)((N + nb - 1) / nb);
-    const LoadFlags load{w.flags};
-    scan_blocksum_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum);
-    GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum, w.ranks);
-    GSB_LAUNCH_CHECK();
+    if (int rc = scan_launch(LoadFlags{w.flags}, N, scan_plan(N, kScanBlocks), w.bsum, w.ranks, s)) return rc;
     totals_kernel<<<1, 1, 0, s>>>(N, w.ranks, counts);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
@@ -401,17 +388,17 @@ extern "C" int gsb_adc_apply(uint32_t N, const GsbMcmcRows *src, const GsbMcmcRo
     if (n_final == 0) return GSB_OK;
     if (!rows_valid(*src) || !rows_valid(*dst) || src->shN_rows != dst->shN_rows) return GSB_E_INVALID;
     Ws w;
-    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, ws_layout(N, workspace, w))) return rc;
     RowsArgs a;
     a.src = *src; a.dst = *dst; a.n_final = n_final; a.map = w.map; a.ranks = w.ranks; a.z = z; a.n_split = n_split;
     a.revised = params->revised_opacity != 0;
     ProfScope ps("adc_apply", s);
-    map_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, w.flags, w.ranks, counts, w.map);
+    map_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, w.flags, w.ranks, counts, w.map);
     GSB_LAUNCH_CHECK();
-    rows_kernel<<<blocks_for(n_final), kThreads, 0, s>>>(a);
+    rows_kernel<<<ceil_div(n_final, kThreads), kThreads, 0, s>>>(a);
     GSB_LAUNCH_CHECK();
     if (a.src.shN_rows) {
-        shn_kernel<<<(n_final + kShnRowsPerBlock - 1) / kShnRowsPerBlock, kThreads, 0, s>>>(a);
+        shn_kernel<<<ceil_div(n_final, kShnRowsPerBlock), kThreads, 0, s>>>(a);
         GSB_LAUNCH_CHECK();
     }
     return GSB_OK;
@@ -430,29 +417,21 @@ extern "C" int gsb_adc_prune_classify(uint32_t N, const float *opacity_raw, uint
     }
     if (!opacity_raw) return GSB_E_INVALID;
     Ws w;
-    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, ws_layout(N, workspace, w))) return rc;
     uint32_t *keys = w.map;
-    uint32_t *hist = reinterpret_cast<uint32_t *>(w.bsum);
-    sel::SelectState *st = static_cast<sel::SelectState *>(workspace);
+    sel::SelectState *st = w.st;
     const bool none = n_prune == 0;
     ProfScope ps("adc_prune_classify", s);
     GSB_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(sel::SelectState), s));
     if (!none) {
-        prune_keys_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, opacity_raw, keys);
+        prune_keys_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, opacity_raw, keys);
         GSB_LAUNCH_CHECK();
-        if (int rc = sel::select_kth(keys, N, n_prune, hist, st, s)) return rc;
+        if (int rc = sel::select_kth(keys, N, n_prune, w.hist, st, s)) return rc;
     }
-    prune_flags_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, keys, st, none, w.flags);
+    prune_flags_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, keys, st, none, w.flags);
     GSB_LAUNCH_CHECK();
-    uint64_t nb = (N + 4095) / 4096;
-    if (nb > kScanBlocks) nb = kScanBlocks;
-    const uint32_t seg = (uint32_t)((N + nb - 1) / nb);
-    const LoadFlags load{w.flags};
-    scan_blocksum_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum);
-    GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<(unsigned)nb, kSortThreads, 0, s>>>(load, N, seg, w.bsum, w.ranks);
-    GSB_LAUNCH_CHECK();
-    prune_ranks_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, n_prune, st, none, w.flags, w.ranks, counts);
+    if (int rc = scan_launch(LoadFlags{w.flags}, N, scan_plan(N, kScanBlocks), w.bsum, w.ranks, s)) return rc;
+    prune_ranks_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, n_prune, st, none, w.flags, w.ranks, counts);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
@@ -468,7 +447,7 @@ extern "C" int gsb_adc_reset_opacity(uint32_t N, float *opacity_raw, float prune
     const float x = 2.0f * prune_opacity;
     const float thr = std::log(x / (1.0f - x));
     ProfScope ps("adc_reset_opacity", s);
-    reset_opacity_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, opacity_raw, thr);
+    reset_opacity_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, opacity_raw, thr);
     GSB_LAUNCH_CHECK();
     if (exp_avg) GSB_CUDA_TRY(cudaMemsetAsync(exp_avg, 0, (size_t)N * sizeof(float), s));
     if (exp_avg_sq) GSB_CUDA_TRY(cudaMemsetAsync(exp_avg_sq, 0, (size_t)N * sizeof(float), s));

@@ -28,9 +28,10 @@
 //    and the box is added to global memory once per CTA.  Where the box does not fit (grid cells much smaller than
 //    the pixel block), the warp sums go to global memory directly -- still one update per (cell, channel) per warp;
 //  * the TV loss and its gradient are one launch: the upstream weight comes from device memory, every gradient
-//    element is written (no zero-fill), and the loss is reduced deterministically (per-CTA partials, the last CTA
-//    sums them in a fixed order) into a device scalar.
+//    element is written (no zero-fill), and the loss is reduced deterministically (gsb_reduce.cuh) into a device
+//    scalar.
 #include "gsb_common.cuh"
+#include "gsb_reduce.cuh"
 
 namespace gsb {
 
@@ -258,20 +259,7 @@ struct TvArgs {
     int L, H, W, N;
 };
 
-__device__ __forceinline__ double bg_block_sum(double v, double *red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-    for (int k = 0; k < kTvThreads / 32; ++k) t += red[k]; // fixed order: deterministic
-    return t;
-}
-
 __global__ void __launch_bounds__(kTvThreads) bilagrid_tv_kernel(const TvArgs a) {
-    __shared__ double red[kTvThreads / 32];
-    __shared__ bool last;
     const int W = a.W, H = a.H, L = a.L, HW = H * W;
     // per-direction 1 / (number of neighbour pairs); a direction of size 1 has none
     const float ix = W > 1 ? 1.f / (float)(L * H * (W - 1)) : 0.f;
@@ -294,25 +282,23 @@ __global__ void __launch_bounds__(kTvThreads) bilagrid_tv_kernel(const TvArgs a)
         if (z < L - 1) g += (v - __ldg(p + HW)) * iz;
         if (a.v_grids) a.v_grids[e] = s * g;
     }
-    const double bx = bg_block_sum((double)sx, red), by = bg_block_sum((double)sy, red), bz = bg_block_sum((double)sz, red);
-    if (threadIdx.x == 0) {
-        a.partials[3 * blockIdx.x + 0] = bx;
-        a.partials[3 * blockIdx.x + 1] = by;
-        a.partials[3 * blockIdx.x + 2] = bz;
-        __threadfence();
-        last = atomicAdd(a.done, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    double tx = 0.0, ty = 0.0, tz = 0.0;
-    for (int b = threadIdx.x; b < (int)gridDim.x; b += kTvThreads) {
-        const volatile double *q = a.partials + 3 * b;
-        tx += q[0]; ty += q[1]; tz += q[2];
-    }
-    tx = bg_block_sum(tx, red); ty = bg_block_sum(ty, red); tz = bg_block_sum(tz, red);
+    double t[3];
+    if (!grid_sum_last<kTvThreads, 3>({(double)sx, (double)sy, (double)sz}, a.partials, a.done, t)) return;
     if (threadIdx.x == 0)
-        *a.loss_out = (float)((tx * (double)ix + ty * (double)iy + tz * (double)iz) / (12.0 * (double)a.N));
+        *a.loss_out = (float)((t[0] * (double)ix + t[1] * (double)iy + t[2] * (double)iz) / (12.0 * (double)a.N));
+}
+
+struct TvWs {
+    unsigned int *done;
+    double *partials; // [kTvMaxBlocks][3]
+};
+
+// the buffers of a workspace at `base` (null: sizing only); returns its size
+static size_t tv_ws_layout(void *base, TvWs &w) {
+    WsLayout l{static_cast<char *>(base)};
+    w.done = l.carve<unsigned int>(1);
+    w.partials = l.carve<double>((size_t)kTvMaxBlocks * 3);
+    return l.bytes;
 }
 
 static int bg_check_shape(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l, uint32_t n_images) {
@@ -365,12 +351,10 @@ extern "C" int gsb_bilagrid_slice_bwd(uint32_t grid_w, uint32_t grid_h, uint32_t
     return GSB_OK;
 }
 
-static unsigned gsb_bilagrid_tv_blocks(uint64_t total) {
-    const uint64_t b = (total + gsb::kTvThreads - 1) / gsb::kTvThreads;
-    return (unsigned)(b < (uint64_t)gsb::kTvMaxBlocks ? b : (uint64_t)gsb::kTvMaxBlocks);
+extern "C" size_t gsb_bilagrid_tv_workspace(void) {
+    gsb::TvWs w;
+    return gsb::tv_ws_layout(nullptr, w);
 }
-
-extern "C" size_t gsb_bilagrid_tv_workspace(void) { return 256 + (size_t)gsb::kTvMaxBlocks * 3 * sizeof(double); }
 
 extern "C" int gsb_bilagrid_tv(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l, uint32_t n_images, const float *grids,
                                const float *grad_weight, float *loss_out, float *v_grids, void *workspace,
@@ -378,19 +362,20 @@ extern "C" int gsb_bilagrid_tv(uint32_t grid_w, uint32_t grid_h, uint32_t grid_l
     using namespace gsb;
     if (bg_check_shape(grid_w, grid_h, grid_l, n_images) != GSB_OK) return GSB_E_INVALID;
     if (!grids || !loss_out) return GSB_E_INVALID;
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_bilagrid_tv_workspace())
-        return GSB_E_WORKSPACE;
+    TvWs w;
+    if (int rc = ws_check(workspace, workspace_bytes, tv_ws_layout(workspace, w))) return rc;
     cudaStream_t st = as_stream(stream);
-    GSB_CUDA_TRY(cudaMemsetAsync(workspace, 0, sizeof(unsigned int), st));
+    GSB_CUDA_TRY(cudaMemsetAsync(w.done, 0, sizeof(unsigned int), st));
     TvArgs a;
     a.grids = grids; a.v_grids = v_grids; a.weight = grad_weight; a.loss_out = loss_out;
-    a.done = reinterpret_cast<unsigned int *>(workspace);
-    a.partials = reinterpret_cast<double *>(reinterpret_cast<char *>(workspace) + 256);
+    a.done = w.done; a.partials = w.partials;
     a.L = (int)grid_l; a.H = (int)grid_h; a.W = (int)grid_w; a.N = (int)n_images;
     a.total = (long long)n_images * 12 * grid_l * grid_h * grid_w;
     {
         ProfScope ps("bilagrid_tv", st);
-        bilagrid_tv_kernel<<<gsb_bilagrid_tv_blocks((uint64_t)a.total), kTvThreads, 0, st>>>(a);
+        uint64_t blocks = ceil_div((uint64_t)a.total, kTvThreads);
+        if (blocks > (uint64_t)kTvMaxBlocks) blocks = kTvMaxBlocks;
+        bilagrid_tv_kernel<<<blocks, kTvThreads, 0, st>>>(a);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;

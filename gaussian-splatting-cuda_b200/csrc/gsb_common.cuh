@@ -45,6 +45,35 @@ static inline uint32_t bit_width_u32(uint32_t n) { // floor(log2 n) + 1, Interse
     return b;
 }
 
+// ceil(n / d), e.g. the CTAs that cover n items at d per CTA
+static inline uint64_t ceil_div(uint64_t n, uint64_t d) { return (n + d - 1) / d; }
+static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Workspace layout.  A stage lists its buffers once, in one function that takes them in order from a WsLayout.  With a
+// null base that function only sizes the workspace (what gsb_*_workspace returns); with the caller's workspace it also
+// points the buffers into it.  The size and the carving therefore cannot disagree.  Every buffer starts on a 256-byte
+// boundary, and no two buffers overlap; `bytes` is the end of the last one.
+struct WsLayout {
+    char *base = nullptr;
+    size_t bytes = 0;
+    // offset of a new buffer of n bytes
+    size_t take(size_t n) {
+        const size_t o = align256(bytes);
+        bytes = o + n;
+        return o;
+    }
+    // a new buffer of `count` T inside the workspace (null while only sizing)
+    template <typename T> T *carve(size_t count) {
+        const size_t o = take(count * sizeof(T));
+        return base ? reinterpret_cast<T *>(base + o) : nullptr;
+    }
+};
+
+// GSB_E_WORKSPACE unless `ws` is a non-null, 256-byte aligned workspace of at least `need` bytes
+static inline int ws_check(const void *ws, size_t bytes, size_t need) {
+    return (!ws || (reinterpret_cast<uintptr_t>(ws) & 255) || bytes < need) ? GSB_E_WORKSPACE : GSB_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // tiny fixed-size linear algebra, templated on the scalar so the per-Gaussian set-up can run
 // in double (it is cancellation-sensitive, see DESIGN.md) while the per-pixel work is float.
@@ -123,7 +152,8 @@ __device__ __forceinline__ M3<float> quat_to_rotmat_norm(float w, float x, float
     return rotmat_raw(w * inv_norm, x * inv_norm, y * inv_norm, z * inv_norm);
 }
 
-// torch's float sigmoid on CUDA (IEEE expf, no fast-math): the ADC flags and the sparsifier compare its values
+// torch's float sigmoid on CUDA (IEEE expf, no fast-math): the MCMC dead mask, the ADC flags and the sparsifier compare
+// its values
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 #endif
 

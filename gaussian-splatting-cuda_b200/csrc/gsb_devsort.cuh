@@ -1,8 +1,7 @@
-// gsb_devsort.cuh -- device-wide sort / scan primitives of the intersect stage, hand-written for sm_90a.
+// gsb_devsort.cuh -- device-wide radix sort of the intersect stage, hand-written for sm_90a.
 //
-// Replaces the library calls of the reference's intersect_tile (cub::DeviceRadixSort::SortPairs,
-// gsplat/IntersectTile.cu:300-314; at::cumsum, gsplat/Intersect.cpp:71) with this repository's own
-// kernels:
+// Replaces the library sort of the reference's intersect_tile (cub::DeviceRadixSort::SortPairs,
+// gsplat/IntersectTile.cu:300-314) with this repository's own kernels:
 //   * radix_count_kernel / radix_scatter_kernel -- stable LSD radix sort of (key, value) pairs, 8 bits per
 //     pass, two launches per pass.  Each CTA owns one contiguous segment; its 32 warps own contiguous
 //     sub-segments and rank their keys with match.any, so equal digits keep their input order.  The
@@ -14,12 +13,11 @@
 //     tiles, or all of them at one depth): the caller therefore writes the values (the identity permutation)
 //     into v0 together with the keys, so that whichever pass runs first -- or, when none does, the run
 //     table itself -- reads a valid permutation from v0.
-//   * scan_blocksum_kernel / scan_apply_kernel -- two-launch inclusive scan (per-CTA sums, then every CTA
-//     adds the sums of its predecessors and scans its own segment).
-// The kernels are stream-ordered and keep no state outside the caller's workspace.
+// The CTA segments are gsb_scan.cuh's.  The kernels are stream-ordered and keep no state outside the caller's
+// workspace.
 #pragma once
 
-#include "gsb_common.cuh"
+#include "gsb_scan.cuh"
 
 namespace gsb {
 
@@ -52,17 +50,6 @@ __device__ __forceinline__ int radix_passes_done(const SortCtl *ctl, int pass) {
 template <typename KeyT>
 __device__ __forceinline__ uint32_t radix_digit(KeyT k, uint32_t shift, uint32_t mask) {
     return (uint32_t)(k >> shift) & mask;
-}
-
-struct SegRange {
-    uint64_t lo, hi;
-};
-__device__ __forceinline__ SegRange cta_segment(uint64_t n, uint32_t seg) {
-    SegRange r;
-    r.lo = (uint64_t)blockIdx.x * seg;
-    r.hi = r.lo + seg < n ? r.lo + seg : n;
-    if (r.lo > n) r.lo = n;
-    return r;
 }
 
 // ---- pass kernel 1: per-CTA digit histogram -------------------------------------------------------------
@@ -189,70 +176,6 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(
             if ((peers >> lane) == 1u) cur[dgt] = base + __popc(peers); // highest lane of the group
         }
         __syncwarp();
-    }
-}
-
-// ---- block-wide inclusive scan of one value per thread (1024 threads) -----------------------------------
-template <typename T>
-__device__ __forceinline__ T block_scan_inclusive(T v, T *s_warp /* [kSortWarps] */, T &total) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const T t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= (uint32_t)o) v += t;
-    }
-    __syncthreads(); // s_warp may still be read by the previous call
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    T add = 0, tot = 0;
-#pragma unroll 8
-    for (int w = 0; w < kSortWarps; ++w) {
-        const T x = s_warp[w];
-        if ((uint32_t)w < warp) add += x;
-        tot += x;
-    }
-    total = tot;
-    return v + add;
-}
-
-// ---- inclusive scan of loader values: Load is `Acc operator()(uint64_t i) const` ---------------------------
-// Instantiated for int32 counts -> int64 (the unsorted path's cum_tiles; Intersect.cpp:71) and, in gsb_mcmc.cu, for
-// 0/1 flags -> int32 ranks and float weights -> a float64 prefix.
-struct LoadI32 {
-    const int32_t *p;
-    __device__ __forceinline__ long long operator()(uint64_t i) const { return p[i]; }
-};
-
-template <typename Load, typename Acc>
-__global__ void __launch_bounds__(kSortThreads) scan_blocksum_kernel(const Load load, uint64_t n, uint32_t seg,
-                                                                     Acc *__restrict__ bsum) {
-    __shared__ Acc s_warp[kSortWarps];
-    const SegRange r = cta_segment(n, seg);
-    Acc acc = 0;
-    for (uint64_t i = r.lo + threadIdx.x; i < r.hi; i += kSortThreads) acc += load(i);
-    Acc tot;
-    block_scan_inclusive<Acc>(acc, s_warp, tot);
-    if (threadIdx.x == 0) bsum[blockIdx.x] = tot;
-}
-
-template <typename Load, typename Acc, typename Out>
-__global__ void __launch_bounds__(kSortThreads) scan_apply_kernel(const Load load, uint64_t n, uint32_t seg,
-                                                                  const Acc *__restrict__ bsum, Out *__restrict__ cum) {
-    __shared__ Acc s_warp[kSortWarps];
-    Acc carry;
-    {
-        Acc part = 0;
-        for (uint32_t bb = threadIdx.x; bb < blockIdx.x; bb += kSortThreads) part += bsum[bb];
-        block_scan_inclusive<Acc>(part, s_warp, carry);
-    }
-    const SegRange r = cta_segment(n, seg);
-    for (uint64_t i0 = r.lo; i0 < r.hi; i0 += kSortThreads) {
-        const uint64_t i = i0 + threadIdx.x;
-        const Acc v = i < r.hi ? load(i) : (Acc)0;
-        Acc tot;
-        const Acc inc = block_scan_inclusive<Acc>(v, s_warp, tot);
-        if (i < r.hi) cum[i] = (Out)(carry + inc);
-        carry += tot;
     }
 }
 

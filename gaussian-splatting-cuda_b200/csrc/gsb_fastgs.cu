@@ -488,27 +488,24 @@ __global__ void __launch_bounds__(kFgsThreads) fgs_back_kernel(const FgsParams p
     }
 }
 
-static inline size_t a256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // layout of the per-primitive buffer (opaque to the caller, carried from forward to backward)
 struct PrimLayout {
     size_t recs, moments, counts, boxes, masks, depths, filt0, filt1, plan, plan_bytes, total;
 };
 static PrimLayout prim_layout(uint32_t N, uint32_t gw, uint32_t gh) {
     PrimLayout l;
-    size_t off = 0;
-    auto take = [&](size_t b) { const size_t o = off; off += a256(b); return o; };
-    l.recs = take((size_t)N * sizeof(GaussRec));
-    l.moments = take((size_t)N * kMomFloats * 4);
-    l.counts = take((size_t)N * 4);
-    l.boxes = take((size_t)N * 8);
-    l.masks = take((size_t)N * 4);
-    l.depths = take((size_t)N * 4);
-    l.filt0 = take((size_t)N * 16);
-    l.filt1 = take((size_t)N * 8);
+    WsLayout w;
+    l.recs = w.take((size_t)N * sizeof(GaussRec));
+    l.moments = w.take((size_t)N * kMomFloats * 4);
+    l.counts = w.take((size_t)N * 4);
+    l.boxes = w.take((size_t)N * 8);
+    l.masks = w.take((size_t)N * 4);
+    l.depths = w.take((size_t)N * 4);
+    l.filt0 = w.take((size_t)N * 16);
+    l.filt1 = w.take((size_t)N * 8);
     l.plan_bytes = isect_plan_ewa_workspace(N, gw, gh);
-    l.plan = take(l.plan_bytes);
-    l.total = off + 256;
+    l.plan = w.take(l.plan_bytes);
+    l.total = align256(w.bytes) + 256;
     return l;
 }
 struct TileLayout {
@@ -518,8 +515,8 @@ static TileLayout tile_layout(uint32_t W, uint32_t H) {
     const uint32_t gw = (W + 15) / 16, gh = (H + 15) / 16;
     TileLayout l;
     l.offsets = 0;
-    l.last_ids = a256(((size_t)gw * gh + 1) * 4);
-    l.total = l.last_ids + a256((size_t)W * H * 4) + 256;
+    l.last_ids = align256(((size_t)gw * gh + 1) * 4);
+    l.total = l.last_ids + align256((size_t)W * H * 4) + 256;
     return l;
 }
 

@@ -30,6 +30,7 @@
 // is ordered by (depth, index) -- the same permutation as the reference's single 46-bit sort, ties included.
 #include "gsb_devsort.cuh"
 #include "gsb_ewa.cuh"
+#include "gsb_scan.cuh"
 
 namespace gsb {
 
@@ -185,35 +186,18 @@ __global__ void __launch_bounds__(kIsectThreads) isect_plan_boxes_kernel(uint64_
 struct RunAcc {
     unsigned long long cnt;
     uint32_t runs;
+    RunAcc() = default;
+    __device__ __forceinline__ RunAcc(int v) : cnt(v), runs(v) {}
     __device__ __forceinline__ RunAcc &operator+=(const RunAcc &o) { cnt += o.cnt; runs += o.runs; return *this; }
+    __device__ __forceinline__ RunAcc operator+(const RunAcc &o) const { RunAcc r = *this; return r += o; }
+    // found by argument-dependent lookup from block_scan_inclusive
+    friend __device__ __forceinline__ RunAcc __shfl_up_sync(unsigned mask, const RunAcc &v, int delta) {
+        RunAcc r;
+        r.cnt = ::__shfl_up_sync(mask, v.cnt, delta);
+        r.runs = ::__shfl_up_sync(mask, v.runs, delta);
+        return r;
+    }
 };
-__device__ __forceinline__ RunAcc operator+(RunAcc a, const RunAcc &b) { a += b; return a; }
-
-__device__ __forceinline__ RunAcc run_shfl_up(RunAcc v, int o) {
-    RunAcc r;
-    r.cnt = __shfl_up_sync(0xffffffffu, v.cnt, o);
-    r.runs = __shfl_up_sync(0xffffffffu, v.runs, o);
-    return r;
-}
-__device__ __forceinline__ RunAcc run_block_scan(RunAcc v, RunAcc *s_warp, RunAcc &total) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const RunAcc t = run_shfl_up(v, o);
-        if (lane >= (uint32_t)o) v += t;
-    }
-    __syncthreads();
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    RunAcc add = {0ull, 0u}, tot = {0ull, 0u};
-    for (int w = 0; w < kSortWarps; ++w) {
-        const RunAcc x = s_warp[w];
-        if ((uint32_t)w < warp) add += x;
-        tot += x;
-    }
-    total = tot;
-    return v + add;
-}
 
 struct RunTable {
     uint32_t *end;  // cumulative number of intersections up to and including this run
@@ -237,26 +221,26 @@ __device__ __forceinline__ const uint32_t *sorted_vals(const SortCtl *ctl, const
     return (radix_passes_done(ctl, 4) & 1) ? v1 : v0;
 }
 
-__global__ void __launch_bounds__(kSortThreads) runs_blocksum_kernel(const SortCtl *__restrict__ ctl,
+__global__ void __launch_bounds__(kScanThreads) runs_blocksum_kernel(const SortCtl *__restrict__ ctl,
                                                                      const uint32_t *__restrict__ v0,
                                                                      const uint32_t *__restrict__ v1,
                                                                      const int32_t *__restrict__ counts, uint64_t n,
                                                                      uint32_t seg, RunAcc *__restrict__ bsum) {
-    __shared__ RunAcc s_warp[kSortWarps];
+    __shared__ RunAcc s_warp[kScanWarps];
     const uint32_t *perm = sorted_vals(ctl, v0, v1);
     const SegRange r = cta_segment(n, seg);
-    RunAcc acc = {0ull, 0u};
-    for (uint64_t i = r.lo + threadIdx.x; i < r.hi; i += kSortThreads) {
+    RunAcc acc = 0;
+    for (uint64_t i = r.lo + threadIdx.x; i < r.hi; i += kScanThreads) {
         const int32_t c = counts[perm[i]];
         acc.cnt += (unsigned long long)c;
         acc.runs += c > 0 ? 1u : 0u;
     }
     RunAcc tot;
-    run_block_scan(acc, s_warp, tot);
+    block_scan_inclusive<RunAcc, kScanWarps>(acc, s_warp, tot);
     if (threadIdx.x == 0) bsum[blockIdx.x] = tot;
 }
 
-__global__ void __launch_bounds__(kSortThreads) runs_build_kernel(SortCtl *__restrict__ ctl,
+__global__ void __launch_bounds__(kScanThreads) runs_build_kernel(SortCtl *__restrict__ ctl,
                                                                   const uint32_t *__restrict__ v0,
                                                                   const uint32_t *__restrict__ v1,
                                                                   const uint32_t *__restrict__ k0,
@@ -266,20 +250,20 @@ __global__ void __launch_bounds__(kSortThreads) runs_build_kernel(SortCtl *__res
                                                                   uint32_t seg, uint32_t nblocks,
                                                                   const RunAcc *__restrict__ bsum, RunTable rt,
                                                                   const uint32_t *__restrict__ masks) {
-    __shared__ RunAcc s_warp[kSortWarps];
+    __shared__ RunAcc s_warp[kScanWarps];
     const bool odd = (radix_passes_done(ctl, 4) & 1) != 0;
     const uint32_t *perm = odd ? v1 : v0;
     const uint32_t *keys = odd ? k1 : k0;
     RunAcc carry;
     {
-        RunAcc part = {0ull, 0u};
-        for (uint32_t bb = threadIdx.x; bb < blockIdx.x; bb += kSortThreads) part += bsum[bb];
-        run_block_scan(part, s_warp, carry);
+        RunAcc part = 0;
+        for (uint32_t bb = threadIdx.x; bb < blockIdx.x; bb += kScanThreads) part += bsum[bb];
+        block_scan_inclusive<RunAcc, kScanWarps>(part, s_warp, carry);
     }
     const SegRange r = cta_segment(n, seg);
-    for (uint64_t i0 = r.lo; i0 < r.hi; i0 += kSortThreads) {
+    for (uint64_t i0 = r.lo; i0 < r.hi; i0 += kScanThreads) {
         const uint64_t i = i0 + threadIdx.x;
-        RunAcc v = {0ull, 0u};
+        RunAcc v = 0;
         uint32_t idx = 0;
         if (i < r.hi) {
             idx = perm[i];
@@ -288,7 +272,7 @@ __global__ void __launch_bounds__(kSortThreads) runs_build_kernel(SortCtl *__res
             v.runs = c > 0 ? 1u : 0u;
         }
         RunAcc tot;
-        const RunAcc inc = run_block_scan(v, s_warp, tot);
+        const RunAcc inc = block_scan_inclusive<RunAcc, kScanWarps>(v, s_warp, tot);
         if (v.runs) {
             const uint32_t k = carry.runs + inc.runs - 1u;
             rt.end[k] = (uint32_t)(carry.cnt + inc.cnt);
@@ -562,13 +546,13 @@ __global__ void __launch_bounds__(kIsectThreads) col_segsum_kernel(const uint32_
     if (acc) atomicAdd(&tot[t], acc); // the tile's intersection count (zeroed before the launch)
 }
 // col_tilescan (one CTA): exclusive scan of the tiles' counts -> first slot of every tile (the tile offsets, a6).
-__global__ void __launch_bounds__(kSortThreads) col_tilescan_kernel(const uint32_t *__restrict__ tot, uint32_t T,
+__global__ void __launch_bounds__(kScanThreads) col_tilescan_kernel(const uint32_t *__restrict__ tot, uint32_t T,
                                                                     uint32_t *__restrict__ toff /* [T + 1] */,
                                                                     int32_t *__restrict__ tile_offsets /*nullable*/,
                                                                     int write_total) {
-    __shared__ uint32_t s_warp[kSortWarps];
+    __shared__ uint32_t s_warp[kScanWarps];
     uint32_t carry = 0;
-    for (uint32_t t0 = 0; t0 < T; t0 += kSortThreads) {
+    for (uint32_t t0 = 0; t0 < T; t0 += kScanThreads) {
         const uint32_t t = t0 + threadIdx.x;
         const uint32_t v = t < T ? tot[t] : 0u;
         uint32_t all;
@@ -635,7 +619,6 @@ __global__ void __launch_bounds__(kIsectThreads) isect_offsets_kernel(uint64_t n
 }
 
 // ---- host-side geometry ------------------------------------------------------------------------------------------
-static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 struct DeviceShape {
     int sms;
@@ -660,20 +643,8 @@ static const DeviceShape &device_shape() {
     return s;
 }
 
-// segment length / CTA count of the 1024-thread sort and scan kernels
-struct SegPlan {
-    uint32_t nblocks, seg;
-};
-static SegPlan seg_plan(uint64_t n) {
-    const DeviceShape &d = device_shape();
-    uint64_t nb = (n + 4095) / 4096;
-    if (nb < 1) nb = 1;
-    if (nb > (uint64_t)d.sms) nb = (uint64_t)d.sms;
-    SegPlan s;
-    s.nblocks = (uint32_t)nb;
-    s.seg = (uint32_t)((n + nb - 1) / nb);
-    return s;
-}
+// segments of the 1024-thread sort and scan kernels: at most one CTA per SM
+static ScanPlan seg_plan(uint64_t n) { return scan_plan(n, (uint32_t)device_shape().sms); }
 
 constexpr uint32_t kMaxWindowTiles = 36 * 1024; // 144 KB of counters at most
 
@@ -721,29 +692,28 @@ struct PlanWs {
     size_t ctl, keys0, keys1, vals0, vals1, boxes, hist, bsum, rt_end, rt_idx, rt_box, rt_key, rt_mask, M, seg, tot, toff,
         chunk_run, total;
 };
-static PlanWs plan_ws(uint64_t n, const BinPlan &b, const SegPlan &sp, bool filter = false) {
+static PlanWs plan_ws(uint64_t n, const BinPlan &b, const ScanPlan &sp, bool filter = false) {
     PlanWs w;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
-    w.ctl = take(sizeof(SortCtl));
-    w.keys0 = take(n * 4); w.keys1 = take(n * 4);
-    w.vals0 = take(n * 4); w.vals1 = take(n * 4);
-    w.boxes = take(n * 8);
-    w.hist = take((size_t)sp.nblocks * kRadixBins * 4);
-    w.bsum = take((size_t)sp.nblocks * sizeof(RunAcc));
-    w.rt_end = take(n * 4); w.rt_idx = take(n * 4); w.rt_box = take(n * 8); w.rt_key = take(n * 4);
-    w.rt_mask = filter ? take(n * 4) : 0;
-    w.M = take((size_t)b.P * b.T_total * 4);
-    w.seg = take((size_t)b.S * b.T_total * 4);
-    w.tot = take((size_t)b.T_total * 4);
-    w.toff = take(((size_t)b.T_total + 1) * 4);
-    w.chunk_run = take(((size_t)b.P + 1) * 4);
-    w.total = off + 256;
+    WsLayout l;
+    w.ctl = l.take(sizeof(SortCtl));
+    w.keys0 = l.take(n * 4); w.keys1 = l.take(n * 4);
+    w.vals0 = l.take(n * 4); w.vals1 = l.take(n * 4);
+    w.boxes = l.take(n * 8);
+    w.hist = l.take((size_t)sp.nblocks * kRadixBins * 4);
+    w.bsum = l.take((size_t)sp.nblocks * sizeof(RunAcc));
+    w.rt_end = l.take(n * 4); w.rt_idx = l.take(n * 4); w.rt_box = l.take(n * 8); w.rt_key = l.take(n * 4);
+    w.rt_mask = filter ? l.take(n * 4) : 0;
+    w.M = l.take((size_t)b.P * b.T_total * 4);
+    w.seg = l.take((size_t)b.S * b.T_total * 4);
+    w.tot = l.take((size_t)b.T_total * 4);
+    w.toff = l.take(((size_t)b.T_total + 1) * 4);
+    w.chunk_run = l.take(((size_t)b.P + 1) * 4);
+    w.total = align256(l.bytes) + 256;
     return w;
 }
 
 template <typename KeyT>
-static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, const SegPlan &sp, int passes,
+static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, const ScanPlan &sp, int passes,
                              uint32_t begin_bit, uint32_t end_bit, const SortCtl *ctl, uint32_t *H, cudaStream_t s) {
     for (int pass = 0; pass < passes; ++pass) {
         const uint32_t shift = begin_bit + 8u * (uint32_t)pass;
@@ -764,7 +734,7 @@ static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uin
 } // namespace gsb
 
 extern "C" size_t gsb_isect_count_workspace(uint64_t n_elements) {
-    const gsb::SegPlan sp = gsb::seg_plan(n_elements);
+    const gsb::ScanPlan sp = gsb::seg_plan(n_elements);
     return gsb::align256((size_t)sp.nblocks * sizeof(long long)) + 256;
 }
 
@@ -783,13 +753,8 @@ extern "C" int gsb_isect_count(uint32_t C, uint32_t N, const float *means2d, con
     isect_count_kernel<<<grid, kIsectThreads, 0, s>>>(n, means2d, radii, tile_size, tile_width, tile_height,
                                                       tiles_per_gauss);
     GSB_LAUNCH_CHECK();
-    const SegPlan sp = seg_plan(n);
     long long *bsum = reinterpret_cast<long long *>(workspace);
-    scan_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{tiles_per_gauss}, n, sp.seg, bsum);
-    GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{tiles_per_gauss}, n, sp.seg, bsum, cum_tiles);
-    GSB_LAUNCH_CHECK();
-    return GSB_OK;
+    return scan_launch(LoadI32{tiles_per_gauss}, n, seg_plan(n), bsum, cum_tiles, s);
 }
 
 extern "C" int gsb_isect_emit(uint32_t C, uint32_t N, const float *means2d, const int32_t *radii,
@@ -814,7 +779,7 @@ extern "C" int gsb_isect_emit(uint32_t C, uint32_t N, const float *means2d, cons
 // Generic stable sort of unsorted (isect_id, flatten_id) pairs on the low 32+tile_bits+cam_bits key bits
 // (IntersectTile.cu:290-328): ceil(bits / 8) passes of the radix kernels of gsb_devsort.cuh.
 extern "C" size_t gsb_isect_sort_workspace(uint64_t n_isects) {
-    const gsb::SegPlan sp = gsb::seg_plan(n_isects);
+    const gsb::ScanPlan sp = gsb::seg_plan(n_isects);
     return gsb::align256(n_isects * 8) + gsb::align256(n_isects * 4) +
            gsb::align256((size_t)sp.nblocks * gsb::kRadixBins * 4) + 256;
 }
@@ -835,7 +800,7 @@ extern "C" int gsb_isect_sort(uint64_t n_isects, uint32_t C, uint32_t tile_width
     const int passes = (int)((end_bit + 7) / 8);
     cudaStream_t s = as_stream(stream);
     ProfScope ps("isect_sort", s);
-    const SegPlan sp = seg_plan(n_isects);
+    const ScanPlan sp = seg_plan(n_isects);
     char *base = reinterpret_cast<char *>(workspace);
     unsigned long long *tmp_k = reinterpret_cast<unsigned long long *>(base);
     uint32_t *tmp_v = reinterpret_cast<uint32_t *>(base + align256(n_isects * 8));
@@ -890,10 +855,9 @@ static int plan_impl(uint32_t C, uint32_t N, const PlanSource &src, const float 
     if (tile_n_bits + cam_n_bits > 32) return GSB_E_INVALID; // Intersect.cpp:50
     if (tile_width > 0xffffu || tile_height > 0xffffu || n > 0x7fffffffull || T64 > 0x7fffffffull) return GSB_E_INVALID;
     const BinPlan bp = bin_plan(C, N, tile_width, tile_height);
-    const SegPlan sp = seg_plan(n);
+    const ScanPlan sp = seg_plan(n);
     const PlanWs w = plan_ws(n, bp, sp, src.ewa());
-    if (!plan_workspace || (reinterpret_cast<uintptr_t>(plan_workspace) & 255) || plan_workspace_bytes < w.total)
-        return GSB_E_WORKSPACE;
+    if (int rc = ws_check(plan_workspace, plan_workspace_bytes, w.total)) return rc;
     char *base = reinterpret_cast<char *>(plan_workspace);
     SortCtl *ctl = reinterpret_cast<SortCtl *>(base + w.ctl);
     uint32_t *k0 = reinterpret_cast<uint32_t *>(base + w.keys0), *k1 = reinterpret_cast<uint32_t *>(base + w.keys1);
@@ -923,9 +887,9 @@ static int plan_impl(uint32_t C, uint32_t N, const PlanSource &src, const float 
     }
     {
         ProfScope ps("isect_runs", s);
-        runs_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(ctl, v0, v1, tiles_per_gauss, n, sp.seg, bsum);
+        runs_blocksum_kernel<<<sp.nblocks, kScanThreads, 0, s>>>(ctl, v0, v1, tiles_per_gauss, n, sp.seg, bsum);
         GSB_LAUNCH_CHECK();
-        runs_build_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(ctl, v0, v1, k0, k1, tiles_per_gauss,
+        runs_build_kernel<<<sp.nblocks, kScanThreads, 0, s>>>(ctl, v0, v1, k0, k1, tiles_per_gauss,
                                                              src.ewa() ? src.boxes : boxes, n, sp.seg, sp.nblocks, bsum,
                                                              rt, src.masks);
         GSB_LAUNCH_CHECK();
@@ -962,7 +926,7 @@ static int plan_impl(uint32_t C, uint32_t N, const PlanSource &src, const float 
         GSB_CUDA_TRY(cudaMemsetAsync(tot, 0, (size_t)bp.T_total * 4, s));
         col_segsum_kernel<<<cgrid, kIsectThreads, 0, s>>>(M, bp.T_total, bp.P, bp.seg_len, seg, tot);
         GSB_LAUNCH_CHECK();
-        col_tilescan_kernel<<<1, kSortThreads, 0, s>>>(tot, bp.T_total, toff, tile_offsets_out, tile_offsets_total);
+        col_tilescan_kernel<<<1, kScanThreads, 0, s>>>(tot, bp.T_total, toff, tile_offsets_out, tile_offsets_total);
         GSB_LAUNCH_CHECK();
         col_apply_kernel<<<cgrid, kIsectThreads, 0, s>>>(M, bp.T_total, bp.P, bp.seg_len, seg, toff);
         GSB_LAUNCH_CHECK();
@@ -979,7 +943,7 @@ static int emit_impl(uint32_t C, uint32_t N, bool filter, const float4 *filt0, c
     if (!plan_workspace || !flatten_ids || !depths) return GSB_E_INVALID;
     if (n_isects > 0x7fffffffull) return GSB_E_INVALID;
     const BinPlan bp = bin_plan(C, N, tile_width, tile_height);
-    const SegPlan sp = seg_plan(n);
+    const ScanPlan sp = seg_plan(n);
     const PlanWs w = plan_ws(n, bp, sp, filter);
     if ((reinterpret_cast<uintptr_t>(plan_workspace) & 255) || plan_workspace_bytes < w.total) return GSB_E_WORKSPACE;
     char *base = const_cast<char *>(reinterpret_cast<const char *>(plan_workspace));

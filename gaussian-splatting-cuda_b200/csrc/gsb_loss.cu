@@ -297,9 +297,15 @@ __global__ void __launch_bounds__(kLossThreads, 3) ssim_l1_kernel(const LossPara
     }
 }
 
+// The workspace: the running sums and the CTA ticket, zeroed together before every launch.
+struct LossCtl {
+    double acc[2];
+    unsigned int done;
+};
+
 } // namespace gsb
 
-extern "C" size_t gsb_ssim_l1_workspace(void) { return 256; }
+extern "C" size_t gsb_ssim_l1_workspace(void) { return gsb::align256(sizeof(gsb::LossCtl)); }
 
 extern "C" int gsb_ssim_l1(uint32_t image_width, uint32_t image_height, const float *renders, const float *target,
                            int target_chw, float lambda_dssim, float grad_scale, float *v_renders, float *loss_out,
@@ -307,17 +313,17 @@ extern "C" int gsb_ssim_l1(uint32_t image_width, uint32_t image_height, const fl
     using namespace gsb;
     if (image_width == 0 || image_height == 0) return GSB_E_INVALID;
     if (!renders || !target || !loss_out) return GSB_E_INVALID;
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_ssim_l1_workspace())
-        return GSB_E_WORKSPACE;
+    if (int rc = ws_check(workspace, workspace_bytes, gsb_ssim_l1_workspace())) return rc;
+    LossCtl *ctl = static_cast<LossCtl *>(workspace);
     cudaStream_t s = as_stream(stream);
-    GSB_CUDA_TRY(cudaMemsetAsync(workspace, 0, 64, s));
+    GSB_CUDA_TRY(cudaMemsetAsync(ctl, 0, sizeof(LossCtl), s));
     LossParams p;
     p.H = image_height; p.W = image_width;
     p.renders = renders; p.target = target;
     p.target_chw = (target_chw & 1) != 0; p.renders_chw = (target_chw & 2) != 0; // GSB_LOSS_TARGET_CHW | GSB_LOSS_RENDERS_CHW
     p.lambda = lambda_dssim; p.grad_scale = grad_scale; p.v_renders = v_renders;
-    p.acc = reinterpret_cast<double *>(workspace);
-    p.done = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(workspace) + 32);
+    p.acc = ctl->acc;
+    p.done = &ctl->done;
     p.loss_out = loss_out;
     // fused_ssim(..., "valid"): the map is cropped by 5 per side only when both sides exceed 10 (fused_ssim.cuh:63-67)
     const bool crop = image_height > 10 && image_width > 10;

@@ -18,14 +18,14 @@
 //                        opacity and scale in a second launch: a sample drawn twice would otherwise let one thread
 //                        read a row another thread has already rewritten.
 //   gsb_mcmc_regularize  scale_reg * mean(exp(scaling_raw)) and opacity_reg * mean(sigmoid(opacity_raw)): gradients
-//                        added into the caller's tensors, losses reduced deterministically (per-CTA partials, the last
-//                        CTA sums them in a fixed order).
+//                        added into the caller's tensors, losses reduced deterministically (gsb_reduce.cuh).
 // Nothing here reads a device value on the host: the dead count and the sample count stay in device memory.
 #include <curand_kernel.h>
 
 #include "gsb_common.cuh"
-#include "gsb_devsort.cuh"
+#include "gsb_reduce.cuh"
 #include "gsb_relocation.cuh"
+#include "gsb_scan.cuh"
 
 namespace gsb {
 
@@ -33,35 +33,23 @@ constexpr int kMcmcThreads = 256;
 constexpr uint32_t kMcmcScanBlocks = 264; // two CTAs of 1024 threads per SM of an H100 SXM
 constexpr uint32_t kRegBlocks = 128;
 
+// One workspace serves every entry point; each uses only its own buffers.
 struct McmcWs {
     unsigned int *done; // regulariser ticket
-    void *bsum;         // [kMcmcScanBlocks] 8-byte block sums / [2 kRegBlocks] regulariser partials
-    void *rows;         // 8 N bytes: flags + ranks, the float64 prefix, or the copy counts
+    double *partials;   // [kRegBlocks][2] regulariser partials
+    void *bsum;         // [kMcmcScanBlocks] 8-byte scan block sums: int64 (dead) or float64 (sample)
+    void *rows;         // 8 N bytes: flags + ranks (dead), the float64 prefix (sample) or the copy counts (apply)
 };
 
-static size_t mcmc_ws_bytes(uint32_t N) { return 256 + (size_t)kMcmcScanBlocks * 8 + (size_t)N * 8; }
-
-static int mcmc_ws(uint32_t N, void *workspace, size_t bytes, McmcWs &w) {
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || bytes < mcmc_ws_bytes(N)) return GSB_E_WORKSPACE;
-    char *b = static_cast<char *>(workspace);
-    w.done = reinterpret_cast<unsigned int *>(b);
-    w.bsum = b + 256;
-    w.rows = b + 256 + (size_t)kMcmcScanBlocks * 8;
-    return GSB_OK;
+// the buffers of a workspace at `base` (null: sizing only); returns its size
+static size_t mcmc_ws_layout(uint32_t N, void *base, McmcWs &w) {
+    WsLayout l{static_cast<char *>(base)};
+    w.done = l.carve<unsigned int>(1);
+    w.partials = l.carve<double>(2 * kRegBlocks);
+    w.bsum = l.carve<char>((size_t)kMcmcScanBlocks * 8);
+    w.rows = l.carve<char>((size_t)N * 8);
+    return l.bytes;
 }
-
-struct ScanPlan {
-    uint32_t nblocks, seg;
-};
-static ScanPlan scan_plan(uint64_t n) {
-    uint64_t nb = (n + 4095) / 4096;
-    if (nb < 1) nb = 1;
-    if (nb > kMcmcScanBlocks) nb = kMcmcScanBlocks;
-    return {(uint32_t)nb, (uint32_t)((n + nb - 1) / nb)};
-}
-
-// torch's sigmoid for float (1 / (1 + exp(-x)) with the IEEE expf, not __expf)
-__device__ __forceinline__ float sigmoid_ieee(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // ---- dead mask and compaction -------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kMcmcThreads) mcmc_mask_kernel(uint32_t N, const float *__restrict__ opacity_raw,
@@ -70,7 +58,7 @@ __global__ void __launch_bounds__(kMcmcThreads) mcmc_mask_kernel(uint32_t N, con
                                                                  float *__restrict__ weights) {
     const uint32_t i = blockIdx.x * kMcmcThreads + threadIdx.x;
     if (i >= N) return;
-    const float op = sigmoid_ieee(opacity_raw[i]);
+    const float op = sigmoid_f(opacity_raw[i]);
     const float4 q = reinterpret_cast<const float4 *>(rotation_raw)[i];
     const float q2 = q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w;
     const bool dead = op <= min_opacity || q2 < 1e-8f;
@@ -94,7 +82,7 @@ struct LoadWeight {
     bool logits;
     __device__ __forceinline__ double operator()(uint64_t i) const {
         const float x = w[i];
-        return (double)(logits ? sigmoid_ieee(x) : x);
+        return (double)(logits ? sigmoid_f(x) : x);
     }
 };
 
@@ -182,7 +170,7 @@ __global__ void __launch_bounds__(kMcmcThreads) mcmc_apply_kernel(const ApplyArg
     if (copies > a.n_max) copies = a.n_max;
     // mcmc.cpp:147-167 (relocate_gs) / :225-245 (add_new_gs)
     float o_new;
-    const float grow = relocation_one(sigmoid_ieee(r.opacity_raw[s]), copies, a.binoms, a.n_max, &o_new);
+    const float grow = relocation_one(sigmoid_f(r.opacity_raw[s]), copies, a.binoms, a.n_max, &o_new);
     const float hi = 1.0f - 1e-7f;
     o_new = o_new < a.min_opacity ? a.min_opacity : (o_new > hi ? hi : o_new); // torch::clamp, NaN kept
     r.opacity_raw[t] = logf(o_new / (1.0f - o_new));
@@ -220,17 +208,6 @@ __global__ void __launch_bounds__(kMcmcThreads) mcmc_writeback_kernel(const Appl
 }
 
 // ---- regularisers -------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double mcmc_block_sum(double v, double *red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-    for (int k = 0; k < kMcmcThreads / 32; ++k) t += red[k]; // fixed order: deterministic
-    return t;
-}
-
 struct RegArgs {
     uint32_t N;
     const float *scaling_raw, *opacity_raw;
@@ -243,8 +220,6 @@ struct RegArgs {
 };
 
 __global__ void __launch_bounds__(kMcmcThreads) mcmc_regularize_kernel(const RegArgs a) {
-    __shared__ double red[kMcmcThreads / 32];
-    __shared__ bool last;
     float se = 0.f, so = 0.f;
     for (uint32_t i = blockIdx.x * kMcmcThreads + threadIdx.x; i < a.N; i += gridDim.x * kMcmcThreads) {
         if (a.v_scaling) {
@@ -256,40 +231,25 @@ __global__ void __launch_bounds__(kMcmcThreads) mcmc_regularize_kernel(const Reg
             }
         }
         if (a.v_opacity) {
-            const float sg = sigmoid_ieee(a.opacity_raw[i]);
+            const float sg = sigmoid_f(a.opacity_raw[i]);
             a.v_opacity[i] += a.opacity_g * (1.0f - sg) * sg; // sigmoid backward: grad * (1 - y) * y
             so += sg;
         }
     }
-    const double be = mcmc_block_sum((double)se, red), bo = mcmc_block_sum((double)so, red);
+    double t[2];
+    if (!grid_sum_last<kMcmcThreads, 2>({(double)se, (double)so}, a.partials, a.done, t)) return;
     if (threadIdx.x == 0) {
-        a.partials[2 * blockIdx.x] = be;
-        a.partials[2 * blockIdx.x + 1] = bo;
-        __threadfence();
-        last = atomicAdd(a.done, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    double te = 0.0, to = 0.0;
-    for (int b = threadIdx.x; b < (int)gridDim.x; b += kMcmcThreads) {
-        const volatile double *q = a.partials + 2 * b;
-        te += q[0];
-        to += q[1];
-    }
-    te = mcmc_block_sum(te, red);
-    to = mcmc_block_sum(to, red);
-    if (threadIdx.x == 0) {
-        a.loss_out[0] = a.v_scaling ? (float)((double)a.scale_reg * te / (3.0 * (double)a.N)) : 0.f;
-        a.loss_out[1] = a.v_opacity ? (float)((double)a.opacity_reg * to / (double)a.N) : 0.f;
+        a.loss_out[0] = a.v_scaling ? (float)((double)a.scale_reg * t[0] / (3.0 * (double)a.N)) : 0.f;
+        a.loss_out[1] = a.v_opacity ? (float)((double)a.opacity_reg * t[1] / (double)a.N) : 0.f;
     }
 }
 
-static unsigned blocks_for(uint64_t n) { return (unsigned)((n + kMcmcThreads - 1) / kMcmcThreads); }
-
 } // namespace gsb
 
-extern "C" size_t gsb_mcmc_workspace(uint32_t N) { return gsb::mcmc_ws_bytes(N); }
+extern "C" size_t gsb_mcmc_workspace(uint32_t N) {
+    gsb::McmcWs w;
+    return gsb::mcmc_ws_layout(N, nullptr, w);
+}
 
 extern "C" int gsb_mcmc_dead(uint32_t N, const float *opacity_raw, const float *rotation_raw, float min_opacity,
                              int32_t *dead_idx, uint32_t *n_dead, float *weights, void *workspace,
@@ -299,20 +259,17 @@ extern "C" int gsb_mcmc_dead(uint32_t N, const float *opacity_raw, const float *
     if (!opacity_raw || !rotation_raw || !dead_idx || !n_dead || !weights) return GSB_E_INVALID;
     if (reinterpret_cast<uintptr_t>(rotation_raw) & 15) return GSB_E_INVALID;
     McmcWs w;
-    if (int rc = mcmc_ws(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, mcmc_ws_layout(N, workspace, w))) return rc;
     cudaStream_t s = as_stream(stream);
     int32_t *flags = static_cast<int32_t *>(w.rows);
     int32_t *ranks = flags + N;
     long long *bsum = static_cast<long long *>(w.bsum);
     ProfScope ps("mcmc_dead", s);
-    mcmc_mask_kernel<<<blocks_for(N), kMcmcThreads, 0, s>>>(N, opacity_raw, rotation_raw, min_opacity, flags, weights);
+    mcmc_mask_kernel<<<ceil_div(N, kMcmcThreads), kMcmcThreads, 0, s>>>(N, opacity_raw, rotation_raw, min_opacity,
+                                                                         flags, weights);
     GSB_LAUNCH_CHECK();
-    const ScanPlan sp = scan_plan(N);
-    scan_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{flags}, N, sp.seg, bsum);
-    GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(LoadI32{flags}, N, sp.seg, bsum, ranks);
-    GSB_LAUNCH_CHECK();
-    mcmc_compact_kernel<<<blocks_for(N), kMcmcThreads, 0, s>>>(N, flags, ranks, dead_idx, n_dead);
+    if (int rc = scan_launch(LoadI32{flags}, N, scan_plan(N, kMcmcScanBlocks), bsum, ranks, s)) return rc;
+    mcmc_compact_kernel<<<ceil_div(N, kMcmcThreads), kMcmcThreads, 0, s>>>(N, flags, ranks, dead_idx, n_dead);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
@@ -324,20 +281,16 @@ extern "C" int gsb_mcmc_sample(uint32_t N, const float *weights, int weights_are
     if (N == 0 || n_samples == 0) return GSB_OK;
     if (!weights || !samples || (!uniforms && !philox)) return GSB_E_INVALID;
     McmcWs w;
-    if (int rc = mcmc_ws(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, mcmc_ws_layout(N, workspace, w))) return rc;
     cudaStream_t s = as_stream(stream);
     double *prefix = static_cast<double *>(w.rows);
     double *bsum = static_cast<double *>(w.bsum);
     const LoadWeight load{weights, weights_are_logits != 0};
     const GsbPhilox ph = philox ? *philox : GsbPhilox{};
     ProfScope ps("mcmc_sample", s);
-    const ScanPlan sp = scan_plan(N);
-    scan_blocksum_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(load, N, sp.seg, bsum);
-    GSB_LAUNCH_CHECK();
-    scan_apply_kernel<<<sp.nblocks, kSortThreads, 0, s>>>(load, N, sp.seg, bsum, prefix);
-    GSB_LAUNCH_CHECK();
-    mcmc_draw_kernel<<<blocks_for(n_samples), kMcmcThreads, 0, s>>>(N, prefix, load, n_samples, n_samples_dev, uniforms, ph,
-                                                                    samples);
+    if (int rc = scan_launch(load, N, scan_plan(N, kMcmcScanBlocks), bsum, prefix, s)) return rc;
+    mcmc_draw_kernel<<<ceil_div(n_samples, kMcmcThreads), kMcmcThreads, 0, s>>>(N, prefix, load, n_samples,
+                                                                                n_samples_dev, uniforms, ph, samples);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
@@ -354,7 +307,7 @@ extern "C" int gsb_mcmc_apply(uint32_t N, const GsbMcmcRows *rows, const int32_t
     if (reinterpret_cast<uintptr_t>(r.rotation_raw) & 15) return GSB_E_INVALID;
     if (!targets && (uint64_t)N + n_samples > 0xffffffffull) return GSB_E_INVALID;
     McmcWs w;
-    if (int rc = mcmc_ws(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, mcmc_ws_layout(N, workspace, w))) return rc;
     cudaStream_t s = as_stream(stream);
     ApplyArgs a;
     a.r = r; a.N = N; a.n_samples = n_samples; a.n_dev = n_samples_dev; a.samples = samples; a.targets = targets;
@@ -362,7 +315,7 @@ extern "C" int gsb_mcmc_apply(uint32_t N, const GsbMcmcRows *rows, const int32_t
     a.counts = static_cast<int32_t *>(w.rows);
     ProfScope ps(targets ? "mcmc_relocate" : "mcmc_grow", s);
     GSB_CUDA_TRY(cudaMemsetAsync(a.counts, 0, (size_t)N * sizeof(int32_t), s));
-    const unsigned nb = blocks_for(n_samples);
+    const unsigned nb = (unsigned)ceil_div(n_samples, kMcmcThreads);
     mcmc_count_kernel<<<nb, kMcmcThreads, 0, s>>>(a);
     GSB_LAUNCH_CHECK();
     mcmc_apply_kernel<<<nb, kMcmcThreads, 0, s>>>(a);
@@ -379,16 +332,16 @@ extern "C" int gsb_mcmc_regularize(uint32_t N, const float *scaling_raw, const f
     if (N == 0) return GSB_OK;
     if (!loss_out || (v_scaling && !scaling_raw) || (v_opacity && !opacity_raw)) return GSB_E_INVALID;
     McmcWs w;
-    if (int rc = mcmc_ws(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, mcmc_ws_layout(N, workspace, w))) return rc;
     cudaStream_t s = as_stream(stream);
     RegArgs a;
     a.N = N; a.scaling_raw = scaling_raw; a.opacity_raw = opacity_raw; a.v_scaling = v_scaling; a.v_opacity = v_opacity;
     a.scale_reg = scale_reg; a.opacity_reg = opacity_reg;
     a.scale_g = scale_reg * (1.0f / (float)(3.0 * N)); // torch divides by a scalar through its reciprocal
     a.opacity_g = opacity_reg * (1.0f / (float)N);
-    a.loss_out = loss_out; a.partials = static_cast<double *>(w.bsum); a.done = w.done;
+    a.loss_out = loss_out; a.partials = w.partials; a.done = w.done;
     GSB_CUDA_TRY(cudaMemsetAsync(w.done, 0, sizeof(unsigned int), s));
-    unsigned nb = blocks_for(N);
+    unsigned nb = (unsigned)ceil_div(N, kMcmcThreads);
     if (nb > kRegBlocks) nb = kRegBlocks;
     ProfScope ps("mcmc_regularize", s);
     mcmc_regularize_kernel<<<nb, kMcmcThreads, 0, s>>>(a);

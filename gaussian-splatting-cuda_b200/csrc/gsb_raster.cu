@@ -659,8 +659,6 @@ __global__ void __launch_bounds__(kPrepThreads) finalize_grads_kernel(
     v_opacities[g] = oo;
 }
 
-static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 static int check_camera(const GsbCamera *cam) {
     if (!cam || !cam->viewmats0 || !cam->Ks) return GSB_E_INVALID;
     if (cam->camera_model != GSB_CAMERA_PINHOLE && cam->camera_model != GSB_CAMERA_FISHEYE)

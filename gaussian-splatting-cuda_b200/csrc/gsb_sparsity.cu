@@ -5,14 +5,15 @@
 //                        u += s - z), where prune_z(x) = (x > x_(k)) * x with x_(k) the k-th smallest of x
 //                        (sort(x)[k - 1]) and 0 when k == 0.  The select is gsb_select.cuh's: the threshold never
 //                        leaves the device.  Elementwise float, bit for bit as torch computes it.
-//   gsb_sparsity_loss    0.5 rho ||s - z + u||^2 into a device scalar (per-CTA double partials summed in a fixed
-//                        order by the last CTA: deterministic) and its gradient rho (s - z + u) s (1 - s) added into
-//                        v_opacity.  rho is read from the device, so one captured graph serves the whole phase; a
-//                        zero rho writes a zero loss and leaves the gradient alone.
+//   gsb_sparsity_loss    0.5 rho ||s - z + u||^2 into a device scalar (reduced deterministically, gsb_reduce.cuh) and
+//                        its gradient rho (s - z + u) s (1 - s) added into v_opacity.  rho is read from the device,
+//                        so one captured graph serves the whole phase; a zero rho writes a zero loss and leaves the
+//                        gradient alone.
 // No fast-math; the elementwise arithmetic uses the explicit _rn intrinsics so that nothing is contracted.
 #include <cmath>
 
 #include "gsb_common.cuh"
+#include "gsb_reduce.cuh"
 #include "gsb_select.cuh"
 
 namespace gsb {
@@ -23,26 +24,21 @@ constexpr uint32_t kLossBlocks = 264;
 
 struct Ws {
     sel::SelectState *st;
-    unsigned int *done;
-    uint32_t *hist;   // [kPasses * kBins]
-    double *partials; // [kLossBlocks]
-    uint32_t *keys;   // [N]
+    unsigned int *done; // loss ticket
+    uint32_t *hist;     // [kPasses * kBins]
+    double *partials;   // [kLossBlocks]
+    uint32_t *keys;     // [N]
 };
 
-static size_t ws_bytes(uint32_t N) { return 256 + sel::kHistBytes + (size_t)kLossBlocks * sizeof(double) + (size_t)N * 4; }
-
-static int ws_carve(uint32_t N, void *workspace, size_t bytes, Ws &w) {
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || bytes < ws_bytes(N)) return GSB_E_WORKSPACE;
-    char *b = static_cast<char *>(workspace);
-    w.st = reinterpret_cast<sel::SelectState *>(b);
-    w.done = reinterpret_cast<unsigned int *>(b + 128);
-    b += 256;
-    w.hist = reinterpret_cast<uint32_t *>(b);
-    b += sel::kHistBytes;
-    w.partials = reinterpret_cast<double *>(b);
-    b += (size_t)kLossBlocks * sizeof(double);
-    w.keys = reinterpret_cast<uint32_t *>(b);
-    return GSB_OK;
+// the buffers of a workspace at `base` (null: sizing only); returns its size
+static size_t ws_layout(uint32_t N, void *base, Ws &w) {
+    WsLayout l{static_cast<char *>(base)};
+    w.st = l.carve<sel::SelectState>(1);
+    w.done = l.carve<unsigned int>(1);
+    w.hist = l.carve<uint32_t>(sel::kHistBytes / sizeof(uint32_t));
+    w.partials = l.carve<double>(kLossBlocks);
+    w.keys = l.carve<uint32_t>(N);
+    return l.bytes;
 }
 
 // zt = s + u (u = 0 when initialising), as an order key
@@ -73,17 +69,6 @@ __global__ void __launch_bounds__(kThreads) update_kernel(uint32_t N, const floa
     u[i] = init ? 0.0f : __fadd_rn(u0, __fsub_rn(s, zi));
 }
 
-__device__ __forceinline__ double block_sum(double v, double *red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-    for (int k = 0; k < kThreads / 32; ++k) t += red[k]; // fixed order: deterministic
-    return t;
-}
-
 struct LossArgs {
     uint32_t N;
     const float *opacity_raw, *z, *u, *rho;
@@ -93,8 +78,6 @@ struct LossArgs {
 };
 
 __global__ void __launch_bounds__(kThreads) loss_kernel(const LossArgs a) {
-    __shared__ double red[kThreads / 32];
-    __shared__ bool last;
     const float rho = *a.rho;
     if (rho == 0.0f) { // no loss this iteration (the prune iteration of a captured phase)
         if (blockIdx.x == 0 && threadIdx.x == 0) a.loss_out[0] = 0.0f;
@@ -109,27 +92,18 @@ __global__ void __launch_bounds__(kThreads) loss_kernel(const LossArgs a) {
         const float g = __fmul_rn(__fmul_rn(__fmul_rn(rho, diff), __fsub_rn(1.0f, s)), s);
         a.v_opacity[i] = __fadd_rn(a.v_opacity[i], g);
     }
-    const double b = block_sum(acc, red);
-    if (threadIdx.x == 0) {
-        a.partials[blockIdx.x] = b;
-        __threadfence();
-        last = atomicAdd(a.done, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    double t = 0.0;
-    for (uint32_t bb = threadIdx.x; bb < gridDim.x; bb += kThreads) t += ((const volatile double *)a.partials)[bb];
-    t = block_sum(t, red);
-    if (threadIdx.x == 0) a.loss_out[0] = (float)((double)__fmul_rn(0.5f, rho) * t);
+    double t[1];
+    if (!grid_sum_last<kThreads, 1>({acc}, a.partials, a.done, t)) return;
+    if (threadIdx.x == 0) a.loss_out[0] = (float)((double)__fmul_rn(0.5f, rho) * t[0]);
 }
-
-static unsigned blocks_for(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 } // namespace sparsity
 } // namespace gsb
 
-extern "C" size_t gsb_sparsity_workspace(uint32_t N) { return gsb::sparsity::ws_bytes(N); }
+extern "C" size_t gsb_sparsity_workspace(uint32_t N) {
+    gsb::sparsity::Ws w;
+    return gsb::sparsity::ws_layout(N, nullptr, w);
+}
 
 extern "C" int gsb_sparsity_update(uint32_t N, const float *opacity_raw, float *z, float *u, uint32_t k,
                                    int initialize, void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
@@ -139,16 +113,16 @@ extern "C" int gsb_sparsity_update(uint32_t N, const float *opacity_raw, float *
     if (N == 0) return GSB_OK;
     if (!opacity_raw || !z || !u) return GSB_E_INVALID;
     Ws w;
-    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, ws_layout(N, workspace, w))) return rc;
     cudaStream_t s = as_stream(stream);
     const bool init = initialize != 0, zero = k == 0;
     ProfScope ps(init ? "sparsity_initialize" : "sparsity_update", s);
     if (!zero) {
-        keys_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, opacity_raw, u, init, w.keys);
+        keys_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, opacity_raw, u, init, w.keys);
         GSB_LAUNCH_CHECK();
         if (int rc = sel::select_kth(w.keys, N, k, w.hist, w.st, s)) return rc;
     }
-    update_kernel<<<blocks_for(N), kThreads, 0, s>>>(N, opacity_raw, z, u, init, zero, w.st);
+    update_kernel<<<ceil_div(N, kThreads), kThreads, 0, s>>>(N, opacity_raw, z, u, init, zero, w.st);
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
@@ -166,11 +140,11 @@ extern "C" int gsb_sparsity_loss(uint32_t N, const float *opacity_raw, const flo
     }
     if (!opacity_raw || !z || !u || !v_opacity) return GSB_E_INVALID;
     Ws w;
-    if (int rc = ws_carve(N, workspace, workspace_bytes, w)) return rc;
+    if (int rc = ws_check(workspace, workspace_bytes, ws_layout(N, workspace, w))) return rc;
     LossArgs a;
     a.N = N; a.opacity_raw = opacity_raw; a.z = z; a.u = u; a.rho = rho; a.v_opacity = v_opacity;
     a.loss_out = loss_out; a.partials = w.partials; a.done = w.done;
-    unsigned nb = blocks_for(N);
+    unsigned nb = (unsigned)ceil_div(N, kThreads);
     if (nb > kLossBlocks) nb = kLossBlocks;
     ProfScope ps("sparsity_loss", s);
     GSB_CUDA_TRY(cudaMemsetAsync(w.done, 0, sizeof(unsigned int), s));

@@ -66,8 +66,9 @@ def test_slice_identity_reproduces_clamped_input(native, cuda_device):
     assert float((out - img.clamp(0, 1)).abs().max()) <= 1e-6
 
 
-@pytest.mark.parametrize("N,X,Y,L", [(200, 16, 16, 8), (3, 12, 9, 4), (2, 5, 1, 3)])
+@pytest.mark.parametrize("N,X,Y,L", [(200, 16, 16, 8), (3, 12, 9, 4), (2, 5, 1, 3), (1, 4, 2, 2)])
 def test_tv_vs_float64_restatement(native, cuda_device, N, X, Y, L):
+    """Grid sizes over the 1024-CTA cap, a partial last CTA, and one CTA (1 x 12 x 16 values)."""
     ns = torch.ops.gsplat_b200
     grids = _grids(N, X, Y, L, N, cuda_device)
     w = torch.tensor([2.5], device=cuda_device)

@@ -337,25 +337,26 @@ def test_training_with_strategy_matches_restatement(native, cuda_device, path):
 
 
 def test_regularizer_losses_and_gradients(native, cuda_device):
-    """~1 M Gaussians (the grid-stride loop and the last-CTA reduction both run): the two loss terms against
-    scale_reg * mean(exp(s)) and opacity_reg * mean(sigmoid(o)) in float64, bit-equal across two runs; the gradients
-    against autograd added onto existing ones."""
-    N = 1_000_003
-    P, _, _ = _params(N, 0, cuda_device, seed=9)
-    s, o = P["scaling_raw"], P["opacity_raw"]
-    # existing gradients of the regularisers' own magnitude, so that the added part keeps its precision
-    v_s0, v_o0 = torch.randn_like(s) * 1e-10, torch.randn_like(o) * 1e-9
-    runs = []
-    for _ in range(2):
-        v_s, v_o = v_s0.clone(), v_o0.clone()
-        loss = _ns().mcmc_regularize(s, o, 0.01, 0.02, v_s, v_o)
-        runs.append((loss.clone(), v_s, v_o))
-    assert torch.equal(runs[0][0], runs[1][0])
-    assert torch.equal(runs[0][1], runs[1][1]) and torch.equal(runs[0][2], runs[1][2])
-    want = torch.stack([0.01 * torch.exp(s.double()).mean(), 0.02 * torch.sigmoid(o.double()).mean()])
-    assert torch.allclose(runs[0][0].double(), want, rtol=1e-6, atol=0)
-    g, _, _ = R.regularizer_grads({"scaling_raw": s, "opacity_raw": o}, 0.01, 0.02)
-    assert rel(runs[0][1] - v_s0, g["scaling_raw"]) < 1e-5 and rel(runs[0][2] - v_o0, g["opacity_raw"]) < 1e-5
+    """200 Gaussians (one CTA) and ~1 M (the grid-stride loop and the last-CTA reduction over the 128-CTA cap): the two
+    loss terms against scale_reg * mean(exp(s)) and opacity_reg * mean(sigmoid(o)) in float64, bit-equal across two
+    runs; the gradients against autograd added onto existing ones."""
+    for N in (200, 1_000_003):
+        P, _, _ = _params(N, 0, cuda_device, seed=9)
+        s, o = P["scaling_raw"], P["opacity_raw"]
+        # existing gradients of the regularisers' own magnitude, so that the added part keeps its precision
+        v_s0, v_o0 = torch.randn_like(s) * 1e-10, torch.randn_like(o) * 1e-9
+        runs = []
+        for _ in range(2):
+            v_s, v_o = v_s0.clone(), v_o0.clone()
+            loss = _ns().mcmc_regularize(s, o, 0.01, 0.02, v_s, v_o)
+            runs.append((loss.clone(), v_s, v_o))
+        assert torch.equal(runs[0][0], runs[1][0]), N
+        assert torch.equal(runs[0][1], runs[1][1]) and torch.equal(runs[0][2], runs[1][2]), N
+        want = torch.stack([0.01 * torch.exp(s.double()).mean(), 0.02 * torch.sigmoid(o.double()).mean()])
+        assert torch.allclose(runs[0][0].double(), want, rtol=1e-6, atol=0), N
+        g, _, _ = R.regularizer_grads({"scaling_raw": s, "opacity_raw": o}, 0.01, 0.02)
+        assert rel(runs[0][1] - v_s0, g["scaling_raw"]) < 1e-5, N
+        assert rel(runs[0][2] - v_o0, g["opacity_raw"]) < 1e-5, N
 
 
 @pytest.mark.parametrize("path", ["gsplat", "fastgs"])

@@ -55,31 +55,32 @@ def test_update_matches_restatement_bitwise(native, cuda_device, N, kind):
 
 
 def test_loss_and_gradient(native, cuda_device):
-    N = 1_000_003
-    o = _opacity(N, "random", cuda_device, seed=5)
-    z, u = R.initialize(o[:, None], 0.6)
-    z, u = R.update_state((o + 0.2)[:, None], z, u, 0.6)
-    z, u = z.flatten().contiguous(), u.flatten().contiguous()
-    rho = torch.full((1,), 5e-4, device=cuda_device)
-    g0 = torch.randn(N, device=cuda_device) * 1e-6
-    runs = []
-    for _ in range(2):
+    """200 Gaussians (one CTA) and ~1 M (the last-CTA reduction over the 264-CTA cap)."""
+    for N in (200, 1_000_003):
+        o = _opacity(N, "random", cuda_device, seed=5)
+        z, u = R.initialize(o[:, None], 0.6)
+        z, u = R.update_state((o + 0.2)[:, None], z, u, 0.6)
+        z, u = z.flatten().contiguous(), u.flatten().contiguous()
+        rho = torch.full((1,), 5e-4, device=cuda_device)
+        g0 = torch.randn(N, device=cuda_device) * 1e-6
+        runs = []
+        for _ in range(2):
+            g = g0.clone()
+            loss = _ns().sparsity_loss(o, z, u, rho, g)
+            runs.append((loss.clone(), g))
+        assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1]), N  # deterministic
+        oo = o.clone().requires_grad_(True)
+        want = R.loss(oo, z, u, 5e-4)
+        want.backward()
+        assert abs(float(runs[0][0]) - float(want)) <= 1e-5 * abs(float(want)), N
+        w = g0 + oo.grad
+        d = (runs[0][1] - w).abs()
+        tol = 8 * EPS * (w.abs() + oo.grad.abs()) + 1e-30
+        assert bool((d <= tol).all()), (N, float((d / tol).max()))
+        # rho == 0: zero loss, gradient untouched
         g = g0.clone()
-        loss = _ns().sparsity_loss(o, z, u, rho, g)
-        runs.append((loss.clone(), g))
-    assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1])  # deterministic
-    oo = o.clone().requires_grad_(True)
-    want = R.loss(oo, z, u, 5e-4)
-    want.backward()
-    assert abs(float(runs[0][0]) - float(want)) <= 1e-5 * abs(float(want))
-    w = g0 + oo.grad
-    d = (runs[0][1] - w).abs()
-    tol = 8 * EPS * (w.abs() + oo.grad.abs()) + 1e-30
-    assert bool((d <= tol).all()), float((d / tol).max())
-    # rho == 0: zero loss, gradient untouched
-    g = g0.clone()
-    loss = _ns().sparsity_loss(o, z, u, torch.zeros(1, device=cuda_device), g)
-    assert float(loss) == 0.0 and torch.equal(g, g0)
+        loss = _ns().sparsity_loss(o, z, u, torch.zeros(1, device=cuda_device), g)
+        assert float(loss) == 0.0 and torch.equal(g, g0), N
 
 
 def _params(N, K, dev, seed, quantised):
