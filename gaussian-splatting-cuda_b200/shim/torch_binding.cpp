@@ -217,6 +217,10 @@ void add_noise(const Tensor &raw_opacities, const Tensor &raw_scales, const Tens
     gsplat::add_noise(raw_opacities, raw_scales, raw_quats, noise, means, (float)current_lr);
 }
 
+void image_metrics(const Tensor &image, const Tensor &target, bool image_hwc, Tensor out) {
+    gsplat::image_metrics(image, target, image_hwc, out);
+}
+
 } // namespace
 
 TORCH_LIBRARY(gsplat_b200, m) {
@@ -252,4 +256,5 @@ TORCH_LIBRARY(gsplat_b200, m) {
     m.def("relocation", &relocation);
     m.def("add_noise(Tensor raw_opacities, Tensor raw_scales, Tensor raw_quats, Tensor noise, Tensor(a!) means, float current_lr) -> ()",
           &add_noise);
+    m.def("image_metrics(Tensor image, Tensor target, bool image_hwc, Tensor(a!) out) -> ()", &image_metrics);
 }

@@ -549,6 +549,22 @@ GSB_API int gsb_adc_prune_classify(uint32_t N, const float *opacity_raw, uint32_
                                    int32_t *counts /*DEVICE [8]*/, void *workspace, size_t workspace_bytes,
                                    gsb_stream_t stream);
 
+/* ---- Evaluation metrics (src/training/metrics/metrics.cpp:17-116, PSNR::compute and SSIM::compute) -------------------
+ * gsb_image_metrics: one view's (psnr, ssim) as float32 into out (DEVICE float[2]), in one launch and with no host
+ * read-back, so a caller can fill [V,2] for V views and read it once.  x = clamp(image, 0, 1), y = target:
+ *   psnr = 20 log10(1 / sqrt(max(mean((x - y)^2), 1e-10))) over all 3 H W values (100 for identical images);
+ *   ssim = mean of the SSIM map over all 3 H W values: 11 x 11 window with zero padding 5 ("same" size, no crop),
+ *          per channel, C1 = 0.01^2, C2 = 0.03^2, sigma^2 = E[x^2] - mu^2.  The window is the reference's gaussian(11,
+ *          1.5), whose float32 taps are exp(-d^2 * 1.125) normalised (its inv_denom evaluates to 1.125).
+ * target is [3,H,W]; image is [3,H,W], or [H,W,3] with GSB_METRICS_IMAGE_HWC in flags.  W, H >= 1 and 3 W H at most
+ * INT32_MAX; images smaller than the window are fine.  The sums are float64 and reduced in an order fixed by W and H:
+ * repeated calls give the same bits.  Workspace: gsb_image_metrics_workspace() bytes, 256-aligned; its ticket is zeroed
+ * on the stream, so the call can be captured in a CUDA graph. */
+enum { GSB_METRICS_IMAGE_HWC = 1 };
+GSB_API size_t gsb_image_metrics_workspace(void);
+GSB_API int gsb_image_metrics(uint32_t W, uint32_t H, const float *image, const float *target, uint32_t flags,
+                              float *out /*DEVICE [2]*/, void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

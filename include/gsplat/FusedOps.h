@@ -161,4 +161,9 @@ at::Tensor sparsity_loss(const at::Tensor opacity_raw, const at::Tensor z, const
 // exactly the n_prune rows of lowest sigmoid(opacity_raw) (ties at the boundary: the first in index order)
 std::tuple<at::Tensor, at::Tensor> sparsity_prune_classify(const at::Tensor opacity_raw, const int64_t n_prune);
 
+// Evaluation metrics of one view (src/training/metrics/metrics.cpp:40-116 after the clamp at :441): (psnr, ssim) of
+// clamp(image, 0, 1) against target [3,H,W] written as float32 into out (a [2] device tensor), no host read-back.
+// image: [3,H,W], or [H,W,3] (the from-world blend's layout, read in place) when image_hwc.
+void image_metrics(const at::Tensor image, const at::Tensor target, const bool image_hwc, at::Tensor out);
+
 } // namespace gsplat
