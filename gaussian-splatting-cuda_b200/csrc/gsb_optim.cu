@@ -90,7 +90,8 @@ extern "C" int gsb_adam_step_dynamic(const GsbAdamGroup *groups, uint32_t n_grou
     for (uint32_t i = 0; i < n_groups; ++i) {
         const GsbAdamGroup &g = groups[i];
         if (g.n == 0 && !dynamic_scalars) continue; // (with dynamic scalars the group index must stay aligned)
-        if (!g.param || !g.grad || !g.exp_avg || !g.exp_avg_sq) return GSB_E_INVALID;
+        // an empty tensor has no storage: a zero-size group kept for its row of the scalar table may hold null pointers
+        if (g.n && (!g.param || !g.grad || !g.exp_avg || !g.exp_avg_sq)) return GSB_E_INVALID;
         AdamGroupDev &d = a.g[a.n_groups++];
         d.param = g.param; d.grad = g.grad; d.exp_avg = g.exp_avg; d.exp_avg_sq = g.exp_avg_sq;
         d.n = g.n;

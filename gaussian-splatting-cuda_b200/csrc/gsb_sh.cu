@@ -35,7 +35,8 @@ __global__ void __launch_bounds__(kShThreads) sh_fwd_kernel(uint32_t M, uint32_t
     sh_basis<DEG>(x, y, z, b);
     const float *c = coeffs + (size_t)e * K * 3;
     float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-    if ((K * 3) % 4 == 0 && NB * 3 % 4 == 0) {
+    // a contiguous view may start at any 4-byte offset (e.g. coeffs[1:]): the 128-bit loads need the base aligned too
+    if ((K * 3) % 4 == 0 && NB * 3 % 4 == 0 && (reinterpret_cast<uintptr_t>(coeffs) & 15) == 0) {
         // 16-byte aligned rows: 128-bit loads (K = 16, deg 3: twelve LDG.128 per element)
         const float4 *c4 = reinterpret_cast<const float4 *>(c);
         float f[NB * 3];
@@ -89,7 +90,8 @@ __global__ void __launch_bounds__(kShThreads) sh_bwd_kernel(uint32_t M, uint32_t
     const float g0 = v_colors[(size_t)e * 3], g1 = v_colors[(size_t)e * 3 + 1], g2 = v_colors[(size_t)e * 3 + 2];
     const float *c = coeffs + (size_t)e * K * 3;
     float w[NB];
-    if ((K * 3) % 4 == 0 && NB * 3 % 4 == 0) {
+    if ((K * 3) % 4 == 0 && NB * 3 % 4 == 0 &&
+        ((reinterpret_cast<uintptr_t>(coeffs) | reinterpret_cast<uintptr_t>(v_coeffs)) & 15) == 0) {
         float4 *vc4 = reinterpret_cast<float4 *>(vc);
         const float4 *c4 = reinterpret_cast<const float4 *>(c);
         float f[NB * 3], o[NB * 3];
