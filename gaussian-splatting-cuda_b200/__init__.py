@@ -274,16 +274,47 @@ class GUTRasterizationFunction(torch.autograd.Function):
         return None, g[0], g[1], g[2], g[3], g[4], v_bg, None, None, None, None, None, None, None, None
 
 
+# gs::training::RenderMode (rasterizer.hpp:25-31) by the names stringToRenderMode accepts, and the blend's channel count
+RENDER_MODES = {"RGB": 3, "D": 1, "ED": 1, "RGB_D": 4, "RGB_ED": 4}
+_RENDER_MODE_IDS = {"RGB": 0, "D": 1, "ED": 2, "RGB_D": 3, "RGB_ED": 4}  # gsplat::RenderMode (FusedOps.h)
+
+
+def _check_render_mode(mode: str) -> str:
+    if mode not in RENDER_MODES:  # stringToRenderMode (rasterizer.hpp:45-57)
+        raise ValueError(f"Invalid render mode: {mode}")
+    return mode
+
+
+def _mode_background(mode: str, bg_color):
+    """The blend's background in a render mode (rasterizer.cpp:276-298)."""
+    if mode == "RGB" or bg_color is None:
+        return bg_color
+    zero = torch.zeros((1, 1), dtype=bg_color.dtype, device=bg_color.device)
+    return zero if RENDER_MODES[mode] == 1 else torch.cat([bg_color, zero], -1)
+
+
+def _split_render(mode: str, renders, alphas):
+    """(image [1,H,W,3] or None, depth [1,H,W,1] or None) of the blend's output (rasterizer.cpp:367-395)."""
+    if mode == "RGB":
+        return renders, None
+    image = None if RENDER_MODES[mode] == 1 else renders[..., :-1]
+    depth = renders if RENDER_MODES[mode] == 1 else renders[..., -1:]
+    if mode in ("ED", "RGB_ED"):
+        depth = depth / alphas.clamp_min(1e-10)
+    return image, depth
+
+
 @dataclass
 class RenderOutput:
-    image: torch.Tensor          # [3, H, W], clamped to [0, 1] (rasterizer.cpp:401)
+    image: torch.Tensor | None   # [3, H, W], clamped to [0, 1] (rasterizer.cpp:401); None in D / ED
     alpha: torch.Tensor          # [1, H, W]
-    render_colors: torch.Tensor  # [1, H, W, 3] unclamped (what the loss gradient flows through)
+    render_colors: torch.Tensor  # [1, H, W, C] unclamped blend output (what the loss gradient flows through), C of the mode
     radii: torch.Tensor          # [N]
     depths: torch.Tensor         # [N]
     means2d: torch.Tensor        # [1, N, 2]
     n_isects: int
     visibility: torch.Tensor     # [N] bool (radii > 0), rasterizer.cpp:419
+    depth: torch.Tensor | None = None  # [1, H, W] accumulated (D, RGB_D) or expected (ED, RGB_ED) depth; None in RGB
 
     @property
     def n_visible(self) -> int:  # host sync; kept out of the render path
@@ -294,8 +325,8 @@ def rasterize(means, quats, scales, opacities, sh_coeffs, sh_degree, viewmat, K,
               scaling_modifier=1.0, tile_size=16, eps2d=0.3, near_plane=0.01, far_plane=10000.0,
               radius_clip=0.0, backend: OpsBackend | None = None, camera_model=PINHOLE, radial_coeffs=None,
               tangential_coeffs=None, thin_prism_coeffs=None,
-              sh_exchange: DeferredSHBackward | None = None, projection=None) -> RenderOutput:
-    """gs::training::rasterize for RenderMode::RGB, perfect pinhole, C == 1 (rasterizer.cpp:46-437).
+              sh_exchange: DeferredSHBackward | None = None, projection=None, render_mode: str = "RGB") -> RenderOutput:
+    """gs::training::rasterize, C == 1 (rasterizer.cpp:46-437).
 
     Inputs are the ACTIVATED parameters (get_means/get_rotation/get_scaling/get_opacity/get_shs of
     SplatData): means [N,3], unit quats [N,4] (w,x,y,z), scales [N,3] > 0, opacities [N] in (0,1),
@@ -303,7 +334,11 @@ def rasterize(means, quats, scales, opacities, sh_coeffs, sh_degree, viewmat, K,
     reference's Camera supplies them (rasterizer.cpp:183-206); camera_model PINHOLE or FISHEYE.
     `projection` = (radii, means2d, depths) replaces the projection step (the op is not differentiable, Ops.h:67):
     parity tests feed two backends the SAME projection so that their intersection lists are identical.
+    render_mode: "RGB", "D", "ED", "RGB_D" or "RGB_ED" (RenderMode).  The depth modes blend the projection's
+    camera-space depths as one more channel (rasterizer.cpp:272-298); the depth is not differentiable (Ops.h:67), so a
+    depth loss reaches the Gaussians through the blend weights only.
     """
+    _check_render_mode(render_mode)
     be = backend or _DEFAULT
     camera = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
                   thin_prism_coeffs=thin_prism_coeffs)
@@ -333,13 +368,19 @@ def rasterize(means, quats, scales, opacities, sh_coeffs, sh_degree, viewmat, K,
     with torch.no_grad():
         _tpg, isect_ids, flatten_ids = be.intersect_tile(means2d, radii, depths, 1, tile_size, tile_w, tile_h, True)
         offsets = be.intersect_offset(isect_ids, 1, tile_w, tile_h)
+    if render_mode != "RGB":
+        depth_col = depths.unsqueeze(-1)                                 # [1, N, 1], no gradient
+        colors = depth_col if RENDER_MODES[render_mode] == 1 else torch.cat([colors, depth_col], -1)
+        bg_color = _mode_background(render_mode, bg_color)
     renders, alphas = GUTRasterizationFunction.apply(be, means, quats, scaled, colors, opacities.unsqueeze(0),
                                                      bg_color, viewmat, K, offsets, flatten_ids, width, height,
                                                      tile_size, camera)
+    image, depth = _split_render(render_mode, renders, alphas)
     return RenderOutput(
-        image=torch.clamp(renders[0].permute(2, 0, 1), 0.0, 1.0), alpha=alphas[0].permute(2, 0, 1),
-        render_colors=renders, radii=radii[0].max(-1).values, depths=depths[0], means2d=means2d,
-        n_isects=int(flatten_ids.shape[0]), visibility=masks[0])
+        image=None if image is None else torch.clamp(image[0].permute(2, 0, 1), 0.0, 1.0),
+        alpha=alphas[0].permute(2, 0, 1), render_colors=renders, radii=radii[0].max(-1).values, depths=depths[0],
+        means2d=means2d, n_isects=int(flatten_ids.shape[0]), visibility=masks[0],
+        depth=None if depth is None else depth[0].permute(2, 0, 1))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -350,19 +391,27 @@ class _FusedGUTFunction(torch.autograd.Function):
     """rasterize_from_world_fused_fwd / _bwd as one autograd node: raw parameters in, image out."""
 
     @staticmethod
-    def forward(ctx, means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, viewmat, K, bg, cfg):
+    def forward(ctx, means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, viewmat, K, bg, cfg, mode):
         sh_degree, scaling_modifier, width, height, eps2d, near, far, clip, camera, capacity = cfg
         needs_bwd = any(t.requires_grad for t in (means, sh0, shN, scaling_raw, rotation_raw, opacity_raw))
         args = (means.detach().contiguous(), sh0.detach().contiguous(), shN.detach().contiguous(),
                 scaling_raw.detach().contiguous(), rotation_raw.detach().contiguous(), opacity_raw.detach().contiguous())
         cam = (camera.get("camera_model", PINHOLE), camera.get("radial_coeffs"), camera.get("tangential_coeffs"),
                camera.get("thin_prism_coeffs"))
-        (renders, alphas, radii, means2d, depths, last_ids, tile_offsets, flatten_ids, workspace,
-         n_isects) = _product_ns().rasterize_from_world_fused_fwd(
-            *args, sh_degree, scaling_modifier, viewmat.contiguous(), K.contiguous(), width, height, eps2d, near, far,
-            clip, bg, cam[0], cam[1], cam[2], cam[3], capacity, needs_bwd)
-        ctx.save_for_backward(*args, viewmat, K, bg if bg is not None else torch.empty(0), radii, tile_offsets,
-                              flatten_ids, workspace, alphas, last_ids)
+        fwd_args = (*args, sh_degree, scaling_modifier, viewmat.contiguous(), K.contiguous(), width, height, eps2d, near,
+                    far, clip, bg, cam[0], cam[1], cam[2], cam[3], capacity, needs_bwd)
+        if mode == "RGB":
+            out = _product_ns().rasterize_from_world_fused_fwd(*fwd_args)
+        else:
+            out = _product_ns().rasterize_from_world_fused_fwd_mode(*fwd_args, _RENDER_MODE_IDS[mode])
+        renders, alphas, radii, means2d, depths, last_ids, tile_offsets, flatten_ids, workspace, n_isects = out
+        if mode == "RGB":
+            ctx.save_for_backward(*args, viewmat, K, bg if bg is not None else torch.empty(0), radii, tile_offsets,
+                                  flatten_ids, workspace, alphas, last_ids)
+        else:
+            ctx.save_for_backward(*args, viewmat, K, bg if bg is not None else torch.empty(0), radii, tile_offsets,
+                                  flatten_ids, workspace, alphas, last_ids, depths)
+        ctx.mode = mode
         ctx.cfg = (sh_degree, scaling_modifier, width, height, cam, bg is not None)
         ctx.mark_non_differentiable(radii, means2d, depths, n_isects)
         return renders, alphas, radii, means2d, depths, n_isects
@@ -370,39 +419,52 @@ class _FusedGUTFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, v_renders, v_alphas, *_):
         (means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, viewmat, K, bg, radii, tile_offsets, flatten_ids,
-         workspace, alphas, last_ids) = ctx.saved_tensors
+         workspace, alphas, last_ids) = ctx.saved_tensors[:15]
         sh_degree, scaling_modifier, width, height, cam, has_bg = ctx.cfg
         if v_alphas is None:
             v_alphas = torch.zeros_like(alphas)
-        g = _product_ns().rasterize_from_world_fused_bwd(
-            means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree, scaling_modifier, viewmat, K, width,
-            height, bg if has_bg else None, cam[0], cam[1], cam[2], cam[3], radii, tile_offsets, flatten_ids, workspace,
-            alphas, last_ids, v_renders.contiguous(), v_alphas.contiguous())
+        bwd_args = (means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree, scaling_modifier, viewmat, K,
+                    width, height, bg if has_bg else None, cam[0], cam[1], cam[2], cam[3], radii, tile_offsets,
+                    flatten_ids, workspace, alphas, last_ids, v_renders.contiguous(), v_alphas.contiguous())
+        if ctx.mode == "RGB":
+            g = _product_ns().rasterize_from_world_fused_bwd(*bwd_args)
+        else:
+            g = _product_ns().rasterize_from_world_fused_bwd_mode(*bwd_args, ctx.saved_tensors[15],
+                                                                  _RENDER_MODE_IDS[ctx.mode])
         v_bg = None
         if has_bg and ctx.needs_input_grad[8]:
             v_bg = (v_renders * (1.0 - alphas)).sum(dim=(-3, -2))
-        return g[0], g[1], (g[2] if g[2].numel() else None), g[3], g[4], g[5], None, None, v_bg, None
+        return g[0], g[1], (g[2] if g[2].numel() else None), g[3], g[4], g[5], None, None, v_bg, None, None
 
 
 @dataclass
 class FusedRenderOutput:
-    render_colors: torch.Tensor  # [1, H, W, 3]
+    render_colors: torch.Tensor  # [1, H, W, C], C = RENDER_MODES[render_mode]
     alpha: torch.Tensor          # [1, H, W, 1]
     radii: torch.Tensor          # [1, N, 2] int32
     means2d: torch.Tensor        # [1, N, 2]
     depths: torch.Tensor         # [1, N]
     n_isects: torch.Tensor       # [1] int64 on the device
     capacity: int                # 0: flatten_ids was sized exactly (one host read-back)
+    render_mode: str = "RGB"
 
     @property
-    def image(self):             # [3, H, W] clamped (rasterizer.cpp:401)
-        return torch.clamp(self.render_colors[0].permute(2, 0, 1), 0.0, 1.0)
+    def image(self):             # [3, H, W] clamped (rasterizer.cpp:401); None in D / ED
+        if self.render_mode == "RGB":
+            return torch.clamp(self.render_colors[0].permute(2, 0, 1), 0.0, 1.0)
+        image, _ = _split_render(self.render_mode, self.render_colors, self.alpha)
+        return None if image is None else torch.clamp(image[0].permute(2, 0, 1), 0.0, 1.0)
+
+    @property
+    def depth(self):             # [1, H, W] as RenderOutput.depth; None in RGB
+        _, depth = _split_render(self.render_mode, self.render_colors, self.alpha)
+        return None if depth is None else depth[0].permute(2, 0, 1)
 
 
 def rasterize_fused(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree, viewmat, K, width, height,
                     bg_color=None, scaling_modifier=1.0, eps2d=0.3, near_plane=0.01, far_plane=10000.0, radius_clip=0.0,
                     camera_model=PINHOLE, radial_coeffs=None, tangential_coeffs=None, thin_prism_coeffs=None,
-                    isect_capacity: int = 0) -> FusedRenderOutput:
+                    isect_capacity: int = 0, render_mode: str = "RGB") -> FusedRenderOutput:
     """gs::training::rasterize for RenderMode::RGB on the RAW SplatData tensors (what Trainer holds as parameters,
     include/core/splat_data.hpp:104-109): means [N,3], sh0 [N,1,3], shN [N,K-1,3], log-scales [N,3], unnormalised
     quaternions [N,4], logit opacities [N,1].  Same image and the same parameter gradients as
@@ -410,15 +472,18 @@ def rasterize_fused(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_
         rasterize(means, normalize(rotation), exp(scaling), sigmoid(opacity), cat(sh0, shN), ...)
 
     through autograd, in two kernels plus the intersect / blend kernels, with no torch glue.  isect_capacity > 0
-    removes the one host read-back (compare `n_isects` with the capacity afterwards)."""
+    removes the one host read-back (compare `n_isects` with the capacity afterwards).  render_mode as in rasterize():
+    bg_color stays [1,3]; the depth modes build the blend's background from it as rasterizer.cpp:276-298 does."""
+    _check_render_mode(render_mode)
     load()
     camera = dict(camera_model=camera_model, radial_coeffs=radial_coeffs, tangential_coeffs=tangential_coeffs,
                   thin_prism_coeffs=thin_prism_coeffs)
     cfg = (int(sh_degree), float(scaling_modifier), int(width), int(height), float(eps2d), float(near_plane),
            float(far_plane), float(radius_clip), camera, int(isect_capacity))
     renders, alphas, radii, means2d, depths, n_isects = _FusedGUTFunction.apply(
-        means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, viewmat, K, bg_color, cfg)
-    return FusedRenderOutput(renders, alphas, radii, means2d, depths, n_isects, int(isect_capacity))
+        means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, viewmat, K, _mode_background(render_mode, bg_color),
+        cfg, render_mode)
+    return FusedRenderOutput(renders, alphas, radii, means2d, depths, n_isects, int(isect_capacity), render_mode)
 
 
 def raw_from_activated(means, quats, scales, opacities, sh_coeffs):

@@ -92,8 +92,10 @@ __device__ __forceinline__ void stage_rows_in(float *s_rows, const float *g_rows
     }
 }
 
-template <int DEG>
-__global__ void __launch_bounds__(kFusedThreads, 5) fused_front_kernel(const FusedParams p) {
+// kColour: the record's channels are the SH colour (RGB, and RGB_D / RGB_ED, whose fourth channel the blend reads from
+// `depths`); otherwise the camera-space depth alone (D / ED: one channel, no SH evaluation).
+template <int DEG, bool kColour>
+__device__ __forceinline__ void fused_front_impl(const FusedParams &p) {
     constexpr int NB = (DEG + 1) * (DEG + 1);
     extern __shared__ __align__(128) float s_rows[]; // [kFusedThreads][(K-1)*3]
     __shared__ FusedCam s_cam;
@@ -138,6 +140,14 @@ __global__ void __launch_bounds__(kFusedThreads, 5) fused_front_kernel(const Fus
     }
     if (bulk) mbar_wait(&s_bar, 0);
     if (!keep) return;
+    if constexpr (!kColour) {
+        const float col[3] = {pr.depth, 0.f, 0.f};
+        float4 v0, v1, v2, v3;
+        make_record(s_cam.cc, mean, quat, scale, opac, col, (int32_t)g, v0, v1, v2, v3);
+        float4 *dst = reinterpret_cast<float4 *>(p.recs + g);
+        dst[0] = v0; dst[1] = v1; dst[2] = v2; dst[3] = v3;
+        return;
+    }
 
     // view-dependent colour (SphericalHarmonicsCUDA.cu:374-481 on dirs = mean - campos; +0.5, clamp: rasterizer.cpp:266)
     float b[NB];
@@ -165,9 +175,18 @@ __global__ void __launch_bounds__(kFusedThreads, 5) fused_front_kernel(const Fus
     float4 *dst = reinterpret_cast<float4 *>(p.recs + g);
     dst[0] = v0; dst[1] = v1; dst[2] = v2; dst[3] = v3;
 }
-
 template <int DEG>
-__global__ void __launch_bounds__(kFusedThreads, 4) fused_back_kernel(const FusedParams p) {
+__global__ void __launch_bounds__(kFusedThreads, 5) fused_front_kernel(const FusedParams p) {
+    fused_front_impl<DEG, true>(p);
+}
+__global__ void __launch_bounds__(kFusedThreads, 5) fused_front_depth_kernel(const FusedParams p) {
+    fused_front_impl<0, false>(p);
+}
+
+// kColour: the colour slots of the moment row route into sh0 / shN (RGB, RGB_D, RGB_ED: the fourth channel's slot,
+// kS_C4, is the depth's and is dropped); otherwise they hold the depth's gradient, which is dropped with sh0 / shN = 0.
+template <int DEG, bool kColour>
+__device__ __forceinline__ void fused_back_impl(const FusedParams &p) {
     constexpr int NB = (DEG + 1) * (DEG + 1);
     extern __shared__ __align__(128) float s_rows[]; // shN rows in, v_shN rows out (each thread owns its row)
     __shared__ FusedCam s_cam;
@@ -222,7 +241,7 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_back_kernel(const Fuse
     float vsh0[3] = {0.f, 0.f, 0.f};
     float *row = s_rows + (size_t)tid * rowf;
     if (tid < cnt) {
-        if (visible) {
+        if (visible && kColour) {
             float b[NB];
             const float dx = mean[0] - s_cam.campos[0], dy = mean[1] - s_cam.campos[1], dz = mean[2] - s_cam.campos[2];
             float x = dx, y = dy, z = dz, inorm = 1.f;
@@ -288,6 +307,13 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_back_kernel(const Fuse
         for (uint32_t i = tid; i < n_floats; i += kFusedThreads) g_out[i] = s_rows[i];
     }
 }
+template <int DEG>
+__global__ void __launch_bounds__(kFusedThreads, 4) fused_back_kernel(const FusedParams p) {
+    fused_back_impl<DEG, true>(p);
+}
+__global__ void __launch_bounds__(kFusedThreads, 4) fused_back_depth_kernel(const FusedParams p) {
+    fused_back_impl<0, false>(p);
+}
 
 static int check_fused(const GsbSplatRaw *sp, const GsbCamera *cam) {
     if (!sp || !cam || !cam->viewmats0 || !cam->Ks) return GSB_E_INVALID;
@@ -341,11 +367,15 @@ extern "C" size_t gsb_fused_workspace(uint32_t N) {
     return ((size_t)N * sizeof(gsb::GaussRec) + 255) / 256 * 256 + ((size_t)N * gsb::kMomFloats * 4 + 255) / 256 * 256 + 256;
 }
 
-extern "C" int gsb_fused_front(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
-                               float eps2d, float near_plane, float far_plane, float radius_clip, int zero_moments,
-                               int32_t *radii, float *means2d, float *depths, void *workspace, size_t workspace_bytes,
-                               gsb_stream_t stream) {
-    using namespace gsb;
+namespace gsb {
+static bool valid_render_mode(int render_mode) { return render_mode >= GSB_RENDER_RGB && render_mode <= GSB_RENDER_RGB_ED; }
+// D / ED blend the depth alone: their records and moment rows carry no colour
+static bool depth_only(int render_mode) { return render_mode == GSB_RENDER_D || render_mode == GSB_RENDER_ED; }
+
+static int fused_front(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
+                       float eps2d, float near_plane, float far_plane, float radius_clip, int zero_moments,
+                       int render_mode, int32_t *radii, float *means2d, float *depths, void *workspace,
+                       size_t workspace_bytes, cudaStream_t s) {
     if (int rc = check_fused(sp, cam)) return rc;
     if (sp->N == 0) return GSB_OK;
     if (!radii || !means2d || !depths) return GSB_E_INVALID;
@@ -358,22 +388,24 @@ extern "C" int gsb_fused_front(const GsbSplatRaw *sp, const GsbCamera *cam, uint
     float *moments = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) +
                                                ((size_t)sp->N * sizeof(GaussRec) + 255) / 256 * 256);
     p.moments = zero_moments ? moments : nullptr;
-    cudaStream_t s = as_stream(stream);
     const uint32_t grid = (sp->N + kFusedThreads - 1) / kFusedThreads;
-    const size_t smem = sp->sh_degree >= 1 ? (size_t)kFusedThreads * (sp->sh_coeffs - 1) * 12 : 0;
     {
         ProfScope ps("fused_front", s);
-        GSB_FUSED_LAUNCH(fused_front_kernel);
+        if (depth_only(render_mode)) {
+            fused_front_depth_kernel<<<grid, kFusedThreads, 0, s>>>(p);
+        } else {
+            const size_t smem = sp->sh_degree >= 1 ? (size_t)kFusedThreads * (sp->sh_coeffs - 1) * 12 : 0;
+            GSB_FUSED_LAUNCH(fused_front_kernel);
+        }
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
 
-extern "C" int gsb_fused_back(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
-                              const int32_t *radii, const void *workspace, size_t workspace_bytes, float *v_means,
-                              float *v_sh0, float *v_shN, float *v_scaling, float *v_rotation, float *v_opacity,
-                              gsb_stream_t stream) {
-    using namespace gsb;
+static int fused_back(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
+                      int render_mode, const int32_t *radii, const void *workspace, size_t workspace_bytes,
+                      float *v_means, float *v_sh0, float *v_shN, float *v_scaling, float *v_rotation,
+                      float *v_opacity, cudaStream_t s) {
     if (int rc = check_fused(sp, cam)) return rc;
     if (sp->N == 0) return GSB_OK;
     if (!radii || !v_means || !v_sh0 || !v_scaling || !v_rotation || !v_opacity) return GSB_E_INVALID;
@@ -389,13 +421,56 @@ extern "C" int gsb_fused_back(const GsbSplatRaw *sp, const GsbCamera *cam, uint3
                                           ((size_t)sp->N * sizeof(GaussRec) + 255) / 256 * 256);
     p.v_means = v_means; p.v_sh0 = v_sh0; p.v_shN = v_shN; p.v_scaling = v_scaling; p.v_rotation = v_rotation;
     p.v_opacity = v_opacity;
-    cudaStream_t s = as_stream(stream);
     const uint32_t grid = (sp->N + kFusedThreads - 1) / kFusedThreads;
+    // the shN gradient rows are staged through shared memory even when they are all zero (D / ED)
     const size_t smem = sp->sh_coeffs > 1 ? (size_t)kFusedThreads * (sp->sh_coeffs - 1) * 12 : 0;
     {
         ProfScope ps("fused_back", s);
-        GSB_FUSED_LAUNCH(fused_back_kernel);
+        if (depth_only(render_mode)) {
+            if (smem > 48 * 1024)
+                GSB_CUDA_TRY(cudaFuncSetAttribute(fused_back_depth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  (int)smem));
+            fused_back_depth_kernel<<<grid, kFusedThreads, smem, s>>>(p);
+        } else {
+            GSB_FUSED_LAUNCH(fused_back_kernel);
+        }
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
+}
+} // namespace gsb
+
+extern "C" int gsb_fused_front(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
+                               float eps2d, float near_plane, float far_plane, float radius_clip, int zero_moments,
+                               int32_t *radii, float *means2d, float *depths, void *workspace, size_t workspace_bytes,
+                               gsb_stream_t stream) {
+    return gsb::fused_front(sp, cam, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, zero_moments,
+                            GSB_RENDER_RGB, radii, means2d, depths, workspace, workspace_bytes, gsb::as_stream(stream));
+}
+
+extern "C" int gsb_fused_front_mode(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width,
+                                    uint32_t image_height, float eps2d, float near_plane, float far_plane,
+                                    float radius_clip, int zero_moments, int render_mode, int32_t *radii,
+                                    float *means2d, float *depths, void *workspace, size_t workspace_bytes,
+                                    gsb_stream_t stream) {
+    if (!gsb::valid_render_mode(render_mode)) return GSB_E_UNSUPPORTED;
+    return gsb::fused_front(sp, cam, image_width, image_height, eps2d, near_plane, far_plane, radius_clip, zero_moments,
+                            render_mode, radii, means2d, depths, workspace, workspace_bytes, gsb::as_stream(stream));
+}
+
+extern "C" int gsb_fused_back(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width, uint32_t image_height,
+                              const int32_t *radii, const void *workspace, size_t workspace_bytes, float *v_means,
+                              float *v_sh0, float *v_shN, float *v_scaling, float *v_rotation, float *v_opacity,
+                              gsb_stream_t stream) {
+    return gsb::fused_back(sp, cam, image_width, image_height, GSB_RENDER_RGB, radii, workspace, workspace_bytes,
+                           v_means, v_sh0, v_shN, v_scaling, v_rotation, v_opacity, gsb::as_stream(stream));
+}
+
+extern "C" int gsb_fused_back_mode(const GsbSplatRaw *sp, const GsbCamera *cam, uint32_t image_width,
+                                   uint32_t image_height, int render_mode, const int32_t *radii, const void *workspace,
+                                   size_t workspace_bytes, float *v_means, float *v_sh0, float *v_shN,
+                                   float *v_scaling, float *v_rotation, float *v_opacity, gsb_stream_t stream) {
+    if (!gsb::valid_render_mode(render_mode)) return GSB_E_UNSUPPORTED;
+    return gsb::fused_back(sp, cam, image_width, image_height, render_mode, radii, workspace, workspace_bytes, v_means,
+                           v_sh0, v_shN, v_scaling, v_rotation, v_opacity, gsb::as_stream(stream));
 }

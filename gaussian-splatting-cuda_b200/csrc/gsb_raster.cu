@@ -44,15 +44,14 @@ constexpr int kBwdPix = 4, kBwdPixSmall = 2;
 // ------------------------------------------------------------------------------------------
 // prep
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kPrepThreads) prep_records_kernel(uint32_t N, const float *__restrict__ means,
-                                                                     const float *__restrict__ quats,
-                                                                     const float *__restrict__ scales,
-                                                                     const float *__restrict__ colors,
-                                                                     const float *__restrict__ opacities,
-                                                                     const float *__restrict__ viewmat,
-                                                                     const float *__restrict__ K,
-                                                                     GaussRec *__restrict__ recs,
-                                                                     float *__restrict__ moments /* nullable */) {
+// colors [N,NC]: the record carries channels 0..2 (NC == 1: channel 0, zeros); channel 3 stays in `colors` and the
+// blend kernels gather it by gid.
+template <int NC>
+__device__ __forceinline__ void prep_records_impl(uint32_t N, const float *__restrict__ means,
+                                                  const float *__restrict__ quats, const float *__restrict__ scales,
+                                                  const float *__restrict__ colors, const float *__restrict__ opacities,
+                                                  const float *__restrict__ viewmat, const float *__restrict__ K,
+                                                  GaussRec *__restrict__ recs, float *__restrict__ moments) {
     __shared__ CamConst cam;
     if (threadIdx.x == 0) cam_const_from(viewmat, K, cam);
     __syncthreads();
@@ -69,10 +68,29 @@ __global__ void __launch_bounds__(kPrepThreads) prep_records_kernel(uint32_t N, 
     const float scale[3] = {scales[(size_t)g * 3], scales[(size_t)g * 3 + 1], scales[(size_t)g * 3 + 2]};
     const float opac = opacities[g];
     float4 v0, v1, v2, v3;
-    const float col[3] = {colors[(size_t)g * 3], colors[(size_t)g * 3 + 1], colors[(size_t)g * 3 + 2]};
+    const float col[3] = {colors[(size_t)g * NC], NC > 1 ? colors[(size_t)g * NC + 1] : 0.f,
+                          NC > 1 ? colors[(size_t)g * NC + 2] : 0.f};
     make_record(cam, mean, quat, scale, opac, col, (int32_t)g, v0, v1, v2, v3);
     float4 *dst = reinterpret_cast<float4 *>(recs + g);
     dst[0] = v0; dst[1] = v1; dst[2] = v2; dst[3] = v3;
+}
+__global__ void __launch_bounds__(kPrepThreads) prep_records_kernel(uint32_t N, const float *__restrict__ means,
+                                                                     const float *__restrict__ quats,
+                                                                     const float *__restrict__ scales,
+                                                                     const float *__restrict__ colors,
+                                                                     const float *__restrict__ opacities,
+                                                                     const float *__restrict__ viewmat,
+                                                                     const float *__restrict__ K,
+                                                                     GaussRec *__restrict__ recs,
+                                                                     float *__restrict__ moments /* nullable */) {
+    prep_records_impl<3>(N, means, quats, scales, colors, opacities, viewmat, K, recs, moments);
+}
+template <int NC>
+__global__ void __launch_bounds__(kPrepThreads) prep_records_nc_kernel(
+    uint32_t N, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ colors, const float *__restrict__ opacities, const float *__restrict__ viewmat,
+    const float *__restrict__ K, GaussRec *__restrict__ recs, float *__restrict__ moments /* nullable */) {
+    prep_records_impl<NC>(N, means, quats, scales, colors, opacities, viewmat, K, recs, moments);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -184,10 +202,12 @@ __device__ __forceinline__ void issue_batch(GaussRec *stage, uint64_t *bar, cons
 // ------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------
-template <bool kGeneral, bool kEwa = false>
-__global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParams p, float *__restrict__ renders,
-                                                                  float *__restrict__ alphas,
-                                                                  int32_t *__restrict__ last_ids) {
+// NC channels per pixel (gsb_raster.cuh, kS_C4): channels 0..2 come from the record, channel 3 from ch3[gid * ch3_stride]
+// (NC == 4 only; one load per culled record, handed to the event loop by a shuffle).
+template <bool kGeneral, bool kEwa, int NC>
+__device__ __forceinline__ void raster_fwd_impl(const TileParams &p, const float *__restrict__ ch3, uint32_t ch3_stride,
+                                                float *__restrict__ renders, float *__restrict__ alphas,
+                                                int32_t *__restrict__ last_ids) {
     constexpr int kPix = kFwdPix, kBatch = kFwdThreads, kStages = 2;
     __shared__ __align__(128) GaussRec s_rec[kStages][kBatch];
     __shared__ __align__(8) uint64_t s_full[kStages];
@@ -198,15 +218,18 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
     const PixelMap<kPix> pm = pixel_map<kPix>(tile_x, tile_y, p.W, p.H);
     const uint32_t tid = threadIdx.x;
     const bool has_bg = p.backgrounds != nullptr;
-    const float bg0 = has_bg ? p.backgrounds[0] : 0.f;
-    const float bg1 = has_bg ? p.backgrounds[1] : 0.f;
-    const float bg2 = has_bg ? p.backgrounds[2] : 0.f;
+    float bg[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) bg[k] = has_bg ? p.backgrounds[k] : 0.f;
 
     if (p.masks != nullptr && !p.masks[tile_id]) { // Fwd.cu:143-150: background only, alpha/last_ids untouched
 #pragma unroll
         for (int i = 0; i < kPix; ++i) {
             const size_t pix = (size_t)pm.y[i] * p.W + pm.x;
-            if (pm.in[i]) { renders[pix * 3] = bg0; renders[pix * 3 + 1] = bg1; renders[pix * 3 + 2] = bg2; }
+            if (pm.in[i]) {
+#pragma unroll
+                for (int k = 0; k < NC; ++k) renders[pix * NC + k] = bg[k];
+            }
         }
         return;
     }
@@ -227,12 +250,14 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
 
     const PixelCoords<kPix> pc = pixel_coords<kGeneral, kPix>(pm, tile_x, tile_y, &s_cm);
     // blend state of the thread's pixels
-    float T[kPix], CR[kPix], CG[kPix], CB[kPix];
+    float T[kPix], CC[kPix][NC];
     int32_t last[kPix];
     bool done[kPix];
 #pragma unroll
     for (int i = 0; i < kPix; ++i) {
-        T[i] = 1.0f; CR[i] = CG[i] = CB[i] = 0.0f;
+        T[i] = 1.0f;
+#pragma unroll
+        for (int k = 0; k < NC; ++k) CC[i][k] = 0.0f;
         last[i] = 0;
         done[i] = !pm.in[i] || !pc.ok[i];
     }
@@ -275,6 +300,10 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
               bool cand = false;
               if (rl < cnt)
                   cand = block_may_pass<kEwa>(rec4[rl * 4], rec4[rl * 4 + 1], rec4[rl * 4 + 2], pc.bx0, pc.bx1, pc.by0, pc.by1);
+              float c4_lane = 0.0f; // channel 3 of the lane's record
+              if constexpr (NC == 4) {
+                  if (cand) c4_lane = ch3[(size_t)__float_as_int(rec4[rl * 4 + 3].w) * ch3_stride];
+              }
               uint32_t cmask = __ballot_sync(0xffffffffu, cand);
               while (cmask) {
                 const int32_t t = c0 + __ffs(cmask) - 1;
@@ -288,6 +317,10 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
                 for (int i = 0; i < kPix; ++i) { pass[i] = e[i].pass && !done[i]; any = any || pass[i]; }
                 if (!__any_sync(0xffffffffu, any)) continue;
                 const float4 q3 = rec4[t * 4 + 3];
+                float col[NC];
+                col[0] = q3.x;
+                if constexpr (NC >= 3) { col[1] = q3.y; col[2] = q3.z; }
+                if constexpr (NC == 4) col[3] = __shfl_sync(0xffffffffu, c4_lane, t - c0);
                 // Every pixel branch-free (the warp executes both sides of a per-pixel branch anyway: most pixels
                 // pass per event).  A pixel that does not contribute gets alpha = 0: T and colour stay.
 #pragma unroll
@@ -304,9 +337,8 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
                     const bool sat = ok && nT <= kMinTransmittance;
                     if (sat) alpha = 0.0f;
                     const float vis = __fmul_rn(alpha, T[i]);
-                    CR[i] = __fmaf_rn(q3.x, vis, CR[i]);
-                    CG[i] = __fmaf_rn(q3.y, vis, CG[i]);
-                    CB[i] = __fmaf_rn(q3.z, vis, CB[i]);
+#pragma unroll
+                    for (int k = 0; k < NC; ++k) CC[i][k] = __fmaf_rn(col[k], vis, CC[i][k]);
                     if (!sat) T[i] = nT;
                     if (ok && !sat) last[i] = batch_start + t;
                     done[i] = done[i] || sat;
@@ -321,18 +353,30 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
     // never retire the CTA with a bulk copy still landing in its shared memory
     if (saturated && b + 1 < n_batches) mbar_wait(&s_full[(b + 1) & 1], (uint32_t)(((b + 1) >> 1) & 1));
 
-    // [H,W,3] rows (gsplat operators) or [3,H,W] planes (fastgs API)
-    const size_t cs = p.chw ? (size_t)p.W * p.H : 1, ps = p.chw ? 1 : 3;
+    // [H,W,NC] rows (gsplat operators) or [3,H,W] planes (fastgs API)
+    const size_t cs = p.chw ? (size_t)p.W * p.H : 1, ps = p.chw ? 1 : NC;
 #pragma unroll
     for (int i = 0; i < kPix; ++i) {
         if (!pm.in[i]) continue;
         const size_t pix = (size_t)pm.y[i] * p.W + pm.x;
         alphas[pix] = 1.0f - T[i];
-        renders[pix * ps] = has_bg ? CR[i] + T[i] * bg0 : CR[i];
-        renders[pix * ps + cs] = has_bg ? CG[i] + T[i] * bg1 : CG[i];
-        renders[pix * ps + 2 * cs] = has_bg ? CB[i] + T[i] * bg2 : CB[i];
+#pragma unroll
+        for (int k = 0; k < NC; ++k) renders[pix * ps + k * cs] = has_bg ? CC[i][k] + T[i] * bg[k] : CC[i][k];
         last_ids[pix] = last[i];
     }
+}
+template <bool kGeneral, bool kEwa = false>
+__global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParams p, float *__restrict__ renders,
+                                                                  float *__restrict__ alphas,
+                                                                  int32_t *__restrict__ last_ids) {
+    raster_fwd_impl<kGeneral, kEwa, 3>(p, nullptr, 0u, renders, alphas, last_ids);
+}
+template <bool kGeneral, int NC>
+__global__ void __launch_bounds__(kFwdThreads) raster_fwd_nc_kernel(const TileParams p, const float *__restrict__ ch3,
+                                                                     uint32_t ch3_stride, float *__restrict__ renders,
+                                                                     float *__restrict__ alphas,
+                                                                     int32_t *__restrict__ last_ids) {
+    raster_fwd_impl<kGeneral, false, NC>(p, ch3, ch3_stride, renders, alphas, last_ids);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -340,11 +384,12 @@ __global__ void __launch_bounds__(kFwdThreads) raster_fwd_kernel(const TileParam
 // ------------------------------------------------------------------------------------------
 
 // Per-pixel state of the backward sweep.
+template <int NC>
 struct BwdPixel {
-    float T;          // running transmittance (restored front-to-back value at the current Gaussian)
-    float bdot;       // (colour accumulated behind) . dL/d(colour)
-    float tfva;       // T_final * (dL/d(alpha) - bg . dL/d(colour))
-    float vr, vg, vb; // dL/d(render colour)
+    float T;     // running transmittance (restored front-to-back value at the current Gaussian)
+    float bdot;  // (colour accumulated behind) . dL/d(colour)
+    float tfva;  // T_final * (dL/d(alpha) - bg . dL/d(colour))
+    float v[NC]; // dL/d(render colour)
     int32_t last;
     bool in;
 };
@@ -355,9 +400,9 @@ struct BwdPixel {
 struct EventWeights {
     float w1, w2, g, fac;
 };
-template <bool kEwa = false>
-__device__ __forceinline__ EventWeights bwd_weights(BwdPixel &s, const PixEval &e, bool pass, float lop, float cr,
-                                                    float cg, float cb) {
+template <bool kEwa, int NC>
+__device__ __forceinline__ EventWeights bwd_weights(BwdPixel<NC> &s, const PixEval &e, bool pass, float lop,
+                                                    const float (&col)[NC]) {
     float rD, ex; // same rounding as the forward
     if constexpr (kEwa) {
         rD = 1.0f;
@@ -380,7 +425,9 @@ __device__ __forceinline__ EventWeights bwd_weights(BwdPixel &s, const PixEval &
     EventWeights w;
     w.fac = __fmul_rn(alpha, s.T);
     // v_alpha = sum_c (c_c T - behind_c / (1-alpha)) v_c + T_final (...) / (1-alpha)     (Bwd.cu:296-316)
-    const float cv = __fmaf_rn(cr, s.vr, __fmaf_rn(cg, s.vg, __fmul_rn(cb, s.vb)));
+    float cv = __fmul_rn(col[NC - 1], s.v[NC - 1]);
+#pragma unroll
+    for (int k = NC - 2; k >= 0; --k) cv = __fmaf_rn(col[k], s.v[k], cv);
     const float v_alpha = __fmaf_rn(s.T, cv, __fmul_rn(ra, __fmaf_rn(s.bdot, -1.0f, s.tfva)));
     s.bdot = __fmaf_rn(w.fac, cv, s.bdot);
     w.g = __fmul_rn(araw_g, v_alpha);
@@ -425,8 +472,8 @@ __device__ __forceinline__ void weight_moments(const float (&w)[kPix], const Pix
 
 // The 16 registers of an event for the warp reduction, lanes 16..31 pre-swapped (see MomentSlot):
 // lane L < 16 holds slot i in R[i], lane L >= 16 holds slot i ^ 8.
-template <bool kEwa, bool kSharedX, int kPix>
-__device__ __forceinline__ void event_registers(const BwdPixel (&s)[kPix], const EventWeights (&w)[kPix],
+template <bool kEwa, bool kSharedX, int kPix, int NC>
+__device__ __forceinline__ void event_registers(const BwdPixel<NC> (&s)[kPix], const EventWeights (&w)[kPix],
                                                 const PixEval (&e)[kPix], const ColTerms (&c)[kSharedX ? 1 : kPix],
                                                 bool hi16, float (&R)[16]) {
     float mA[6], mB[6], gs;
@@ -457,24 +504,23 @@ __device__ __forceinline__ void event_registers(const BwdPixel (&s)[kPix], const
     R[8] = hi16 ? gs : mB[0];
 #pragma unroll
     for (int k = 1; k < 6; ++k) { R[k] = mA[k]; R[k + 8] = mB[k]; }
-    float cr = 0.0f, cg = 0.0f, cb = 0.0f;
+    float cs[4] = {0.0f, 0.0f, 0.0f, 0.0f}; // channels beyond NC stay zero
 #pragma unroll
     for (int i = 0; i < kPix; ++i) {
-        cr += w[i].fac * s[i].vr;
-        cg += w[i].fac * s[i].vg;
-        cb += w[i].fac * s[i].vb;
+#pragma unroll
+        for (int k = 0; k < NC; ++k) cs[k] += w[i].fac * s[i].v[k];
     }
-    R[6] = hi16 ? cg : cr; R[14] = hi16 ? cr : cg; // slots kS_CR / kS_CG
-    R[7] = hi16 ? 0.0f : cb; R[15] = hi16 ? cb : 0.0f; // slots kS_CB / kS_PAD
+    R[6] = hi16 ? cs[1] : cs[0]; R[14] = hi16 ? cs[0] : cs[1]; // slots kS_CR / kS_CG
+    R[7] = hi16 ? cs[3] : cs[2]; R[15] = hi16 ? cs[2] : cs[3]; // slots kS_CB / kS_PAD (= kS_C4)
 }
 
-template <bool kGeneral, bool kEwa, int kPix>
-__global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams p,
-                                                                const float *__restrict__ render_alphas,
-                                                                const int32_t *__restrict__ last_ids,
-                                                                const float *__restrict__ v_render_colors,
-                                                                const float *__restrict__ v_render_alphas,
-                                                                float *__restrict__ moments) {
+template <bool kGeneral, bool kEwa, int kPix, int NC>
+__device__ __forceinline__ void raster_bwd_impl(const TileParams &p, const float *__restrict__ ch3, uint32_t ch3_stride,
+                                                const float *__restrict__ render_alphas,
+                                                const int32_t *__restrict__ last_ids,
+                                                const float *__restrict__ v_render_colors,
+                                                const float *__restrict__ v_render_alphas,
+                                                float *__restrict__ moments) {
     // Three stages; a stage is filled through its "full" mbarrier (TMA byte count) and released through its "empty"
     // mbarrier (one arrival per warp): no CTA-wide barrier in the loop, a warp with nothing to do in a batch runs ahead
     // of its neighbour instead of waiting at a two-stage / __syncthreads ring.
@@ -496,19 +542,24 @@ __global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams
                                                                                      : p.tile_offsets[tile_id + 1],
                                   (int32_t)p.cap);
 
-    float bg[3] = {0.f, 0.f, 0.f};
-    if (p.backgrounds) { bg[0] = p.backgrounds[0]; bg[1] = p.backgrounds[1]; bg[2] = p.backgrounds[2]; }
+    float bg[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) bg[k] = 0.f;
+    if (p.backgrounds) {
+#pragma unroll
+        for (int k = 0; k < NC; ++k) bg[k] = p.backgrounds[k];
+    }
 
     if constexpr (kGeneral) {
         if (tid == 0) tile_cam_build(p, s_cm);
         __syncthreads();
     }
     const PixelCoords<kPix> pc = pixel_coords<kGeneral, kPix>(pm, tile_x, tile_y, &s_cm);
-    BwdPixel s[kPix];
+    BwdPixel<NC> s[kPix];
     int32_t wmax = -1;
 #pragma unroll
     for (int i = 0; i < kPix; ++i) {
-        BwdPixel &r = s[i];
+        BwdPixel<NC> &r = s[i];
         r.in = pm.in[i] && pc.ok[i];
         r.bdot = 0.0f;
         if (r.in) {
@@ -516,13 +567,18 @@ __global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams
             const float Tf = 1.0f - render_alphas[pix];
             r.T = Tf;
             r.last = last_ids[pix];
-            const size_t cs = p.chw ? (size_t)p.W * p.H : 1, ps = p.chw ? 1 : 3;
-            r.vr = v_render_colors[pix * ps]; r.vg = v_render_colors[pix * ps + cs]; r.vb = v_render_colors[pix * ps + 2 * cs];
+            const size_t cs = p.chw ? (size_t)p.W * p.H : 1, ps = p.chw ? 1 : NC;
+#pragma unroll
+            for (int k = 0; k < NC; ++k) r.v[k] = v_render_colors[pix * ps + k * cs];
             const float va = v_render_alphas[pix];
-            const float bgd = bg[0] * r.vr + bg[1] * r.vg + bg[2] * r.vb;
+            float bgd = bg[0] * r.v[0];
+#pragma unroll
+            for (int k = 1; k < NC; ++k) bgd = bgd + bg[k] * r.v[k];
             r.tfva = Tf * va - Tf * bgd; // Bwd.cu:307-316
         } else {
-            r.T = 1.f; r.last = -1; r.vr = r.vg = r.vb = 0.f; r.tfva = 0.f;
+            r.T = 1.f; r.last = -1; r.tfva = 0.f;
+#pragma unroll
+            for (int k = 0; k < NC; ++k) r.v[k] = 0.f;
         }
         wmax = max(wmax, r.last);
     }
@@ -578,6 +634,10 @@ __global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams
           bool cand = false;
           if (rl >= t_first && rl < cnt)
               cand = block_may_pass<kEwa>(rec4[rl * 4], rec4[rl * 4 + 1], rec4[rl * 4 + 2], pc.bx0, pc.bx1, pc.by0, pc.by1);
+          float c4_lane = 0.0f; // channel 3 of the lane's record
+          if constexpr (NC == 4) {
+              if (cand) c4_lane = ch3[(size_t)__float_as_int(rec4[rl * 4 + 3].w) * ch3_stride];
+          }
           uint32_t cmask = __ballot_sync(0xffffffffu, cand);
           while (cmask) {
             const int32_t t = c0 + __ffs(cmask) - 1;
@@ -595,21 +655,30 @@ __global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams
             }
             if (!__any_sync(0xffffffffu, any)) continue;
             const float4 q3 = rec4[t * 4 + 3];
+            float col[NC];
+            col[0] = q3.x;
+            if constexpr (NC >= 3) { col[1] = q3.y; col[2] = q3.z; }
+            if constexpr (NC == 4) col[3] = __shfl_sync(0xffffffffu, c4_lane, t - c0);
             // A record often covers only part of the warp's 16 rows: a pixel index that no lane passes gets zero
             // weights and keeps its state, exactly what bwd_weights would give it, without the MUFU work.
             EventWeights w[kPix];
 #pragma unroll
             for (int i = 0; i < kPix; ++i) {
-                if (__any_sync(0xffffffffu, pass[i])) w[i] = bwd_weights<kEwa>(s[i], e[i], pass[i], q2.z, q3.x, q3.y, q3.z);
+                if (__any_sync(0xffffffffu, pass[i])) w[i] = bwd_weights<kEwa, NC>(s[i], e[i], pass[i], q2.z, col);
                 else w[i] = EventWeights{0.0f, 0.0f, 0.0f, 0.0f};
             }
             float R[16];
-            event_registers<kEwa, !kGeneral, kPix>(s, w, e, c, hi16, R);
+            event_registers<kEwa, !kGeneral, kPix, NC>(s, w, e, c, hi16, R);
             butterfly16_preswapped(R);
             if ((tid & 1) == 0) {
                 const uint32_t slot = (tid & 31) >> 1;
+                // slots without a channel: the pad at NC == 3, kS_CG / kS_CB / the pad at NC == 1
+                bool live = true;
+                if constexpr (NC == 3) live = slot != (uint32_t)kS_PAD;
+                if constexpr (NC == 1)
+                    live = slot != (uint32_t)kS_PAD && slot != (uint32_t)kS_CG && slot != (uint32_t)kS_CB;
                 // EWA records: slots 8..13 (the denominator moments) do not exist
-                if (slot != (uint32_t)kS_PAD && !(kEwa && slot >= 8u && slot != (uint32_t)kS_CG))
+                if (live && !(kEwa && slot >= 8u && slot != (uint32_t)kS_CG))
                     red_add_f32(moments + (size_t)__float_as_int(q3.w) * kMomFloats + slot, R[0]);
             }
           }
@@ -618,11 +687,33 @@ __global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams
         if ((tid & 31) == 0) mbar_arrive(&s_empty[st]); // this warp is done with stage `st`
     }
 }
+template <bool kGeneral, bool kEwa, int kPix>
+__global__ void __launch_bounds__(256 / kPix) raster_bwd_kernel(const TileParams p,
+                                                                const float *__restrict__ render_alphas,
+                                                                const int32_t *__restrict__ last_ids,
+                                                                const float *__restrict__ v_render_colors,
+                                                                const float *__restrict__ v_render_alphas,
+                                                                float *__restrict__ moments) {
+    raster_bwd_impl<kGeneral, kEwa, kPix, 3>(p, nullptr, 0u, render_alphas, last_ids, v_render_colors, v_render_alphas,
+                                             moments);
+}
+template <bool kGeneral, int kPix, int NC>
+__global__ void __launch_bounds__(256 / kPix) raster_bwd_nc_kernel(const TileParams p, const float *__restrict__ ch3,
+                                                                   uint32_t ch3_stride,
+                                                                   const float *__restrict__ render_alphas,
+                                                                   const int32_t *__restrict__ last_ids,
+                                                                   const float *__restrict__ v_render_colors,
+                                                                   const float *__restrict__ v_render_alphas,
+                                                                   float *__restrict__ moments) {
+    raster_bwd_impl<kGeneral, false, kPix, NC>(p, ch3, ch3_stride, render_alphas, last_ids, v_render_colors,
+                                               v_render_alphas, moments);
+}
 
 // ------------------------------------------------------------------------------------------
 // finalize: moments -> gradients (chain rule once per Gaussian, float32: see FT below)
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kPrepThreads) finalize_grads_kernel(
+template <int NC>
+__device__ __forceinline__ void finalize_grads_impl(
     uint32_t N, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
     const float *__restrict__ opacities, const float *__restrict__ viewmat, const float *__restrict__ K,
     const GaussRec *__restrict__ recs, const float *__restrict__ moments, float *__restrict__ v_means,
@@ -643,7 +734,9 @@ __global__ void __launch_bounds__(kPrepThreads) finalize_grads_kernel(
             m[i * 4] = v.x; m[i * 4 + 1] = v.y; m[i * 4 + 2] = v.z; m[i * 4 + 3] = v.w;
         }
     }
-    v_colors[(size_t)g * 3] = m[kS_CR]; v_colors[(size_t)g * 3 + 1] = m[kS_CG]; v_colors[(size_t)g * 3 + 2] = m[kS_CB];
+    v_colors[(size_t)g * NC] = m[kS_CR];
+    if constexpr (NC >= 3) { v_colors[(size_t)g * NC + 1] = m[kS_CG]; v_colors[(size_t)g * NC + 2] = m[kS_CB]; }
+    if constexpr (NC == 4) v_colors[(size_t)g * NC + 3] = m[kS_C4];
     float om[3], oq[4], os[3], oo;
     {
         const float mean[3] = {means[(size_t)g * 3], means[(size_t)g * 3 + 1], means[(size_t)g * 3 + 2]};
@@ -657,6 +750,26 @@ __global__ void __launch_bounds__(kPrepThreads) finalize_grads_kernel(
     v_scales[(size_t)g * 3] = os[0]; v_scales[(size_t)g * 3 + 1] = os[1]; v_scales[(size_t)g * 3 + 2] = os[2];
     reinterpret_cast<float4 *>(v_quats)[g] = make_float4(oq[0], oq[1], oq[2], oq[3]);
     v_opacities[g] = oo;
+}
+__global__ void __launch_bounds__(kPrepThreads) finalize_grads_kernel(
+    uint32_t N, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ opacities, const float *__restrict__ viewmat, const float *__restrict__ K,
+    const GaussRec *__restrict__ recs, const float *__restrict__ moments, float *__restrict__ v_means,
+    float *__restrict__ v_quats, float *__restrict__ v_scales, float *__restrict__ v_colors,
+    float *__restrict__ v_opacities) {
+    finalize_grads_impl<3>(N, means, quats, scales, opacities, viewmat, K, recs, moments, v_means, v_quats, v_scales,
+                           v_colors, v_opacities);
+}
+// v_colors [N,NC]
+template <int NC>
+__global__ void __launch_bounds__(kPrepThreads) finalize_grads_nc_kernel(
+    uint32_t N, const float *__restrict__ means, const float *__restrict__ quats, const float *__restrict__ scales,
+    const float *__restrict__ opacities, const float *__restrict__ viewmat, const float *__restrict__ K,
+    const GaussRec *__restrict__ recs, const float *__restrict__ moments, float *__restrict__ v_means,
+    float *__restrict__ v_quats, float *__restrict__ v_scales, float *__restrict__ v_colors,
+    float *__restrict__ v_opacities) {
+    finalize_grads_impl<NC>(N, means, quats, scales, opacities, viewmat, K, recs, moments, v_means, v_quats, v_scales,
+                            v_colors, v_opacities);
 }
 
 static int check_camera(const GsbCamera *cam) {
@@ -713,14 +826,30 @@ static void fill_tiles(TileParams &p, uint64_t n_isects, uint32_t cap, int close
     p.tile_offsets = tile_offsets; p.flatten_ids = flatten_ids;
     fill_camera(p, cam);
 }
-static int launch_fwd(const TileParams &p, const GsbCamera *cam, float *renders, float *alphas, int32_t *last_ids,
-                      cudaStream_t s) {
+// Channel 3 of an NC == 4 blend: ch3[gid * stride] (the caller's colors[:, 3], or the fused front's depths).
+struct Chan3 {
+    const float *ptr;
+    uint32_t stride;
+};
+template <int NC>
+static int launch_fwd(const TileParams &p, const GsbCamera *cam, Chan3 c3, float *renders, float *alphas,
+                      int32_t *last_ids, cudaStream_t s) {
     {
         ProfScope ps("raster_fwd", s);
-        if (general_camera(cam))
-            raster_fwd_kernel<true><<<p.tile_w * p.tile_h, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
-        else
-            raster_fwd_kernel<false><<<p.tile_w * p.tile_h, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
+        const uint32_t tiles = p.tile_w * p.tile_h;
+        if constexpr (NC == 3) {
+            if (general_camera(cam))
+                raster_fwd_kernel<true><<<tiles, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
+            else
+                raster_fwd_kernel<false><<<tiles, kFwdThreads, 0, s>>>(p, renders, alphas, last_ids);
+        } else {
+            if (general_camera(cam))
+                raster_fwd_nc_kernel<true, NC><<<tiles, kFwdThreads, 0, s>>>(p, c3.ptr, c3.stride, renders, alphas,
+                                                                             last_ids);
+            else
+                raster_fwd_nc_kernel<false, NC><<<tiles, kFwdThreads, 0, s>>>(p, c3.ptr, c3.stride, renders, alphas,
+                                                                              last_ids);
+        }
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
@@ -743,27 +872,42 @@ static uint32_t bwd_wide_min_tiles() {
     }();
     return n;
 }
-template <bool kGeneral, bool kEwa>
-static void launch_bwd_kernel(const TileParams &p, const float *render_alphas, const int32_t *last_ids,
+template <bool kGeneral, bool kEwa, int NC = 3>
+static void launch_bwd_kernel(const TileParams &p, Chan3 c3, const float *render_alphas, const int32_t *last_ids,
                               const float *v_render_colors, const float *v_render_alphas, float *moments,
                               cudaStream_t s) {
     const uint32_t tiles = p.tile_w * p.tile_h;
-    if (tiles >= bwd_wide_min_tiles())
-        raster_bwd_kernel<kGeneral, kEwa, kBwdPix><<<tiles, 256 / kBwdPix, 0, s>>>(p, render_alphas, last_ids,
-                                                                                  v_render_colors, v_render_alphas,
-                                                                                  moments);
-    else
-        raster_bwd_kernel<kGeneral, kEwa, kBwdPixSmall><<<tiles, 256 / kBwdPixSmall, 0, s>>>(
-            p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments);
+    const bool wide = tiles >= bwd_wide_min_tiles();
+    if constexpr (NC == 3) {
+        if (wide)
+            raster_bwd_kernel<kGeneral, kEwa, kBwdPix><<<tiles, 256 / kBwdPix, 0, s>>>(p, render_alphas, last_ids,
+                                                                                      v_render_colors, v_render_alphas,
+                                                                                      moments);
+        else
+            raster_bwd_kernel<kGeneral, kEwa, kBwdPixSmall><<<tiles, 256 / kBwdPixSmall, 0, s>>>(
+                p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments);
+    } else {
+        static_assert(!kEwa, "EWA records carry three channels");
+        if (wide)
+            raster_bwd_nc_kernel<kGeneral, kBwdPix, NC><<<tiles, 256 / kBwdPix, 0, s>>>(
+                p, c3.ptr, c3.stride, render_alphas, last_ids, v_render_colors, v_render_alphas, moments);
+        else
+            raster_bwd_nc_kernel<kGeneral, kBwdPixSmall, NC><<<tiles, 256 / kBwdPixSmall, 0, s>>>(
+                p, c3.ptr, c3.stride, render_alphas, last_ids, v_render_colors, v_render_alphas, moments);
+    }
 }
-static int launch_bwd(const TileParams &p, const GsbCamera *cam, const float *render_alphas, const int32_t *last_ids,
-                      const float *v_render_colors, const float *v_render_alphas, float *moments, cudaStream_t s) {
+template <int NC>
+static int launch_bwd(const TileParams &p, const GsbCamera *cam, Chan3 c3, const float *render_alphas,
+                      const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
+                      float *moments, cudaStream_t s) {
     {
         ProfScope ps("raster_bwd", s);
         if (general_camera(cam))
-            launch_bwd_kernel<true, false>(p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, s);
+            launch_bwd_kernel<true, false, NC>(p, c3, render_alphas, last_ids, v_render_colors, v_render_alphas,
+                                               moments, s);
         else
-            launch_bwd_kernel<false, false>(p, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, s);
+            launch_bwd_kernel<false, false, NC>(p, c3, render_alphas, last_ids, v_render_colors, v_render_alphas,
+                                                moments, s);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
@@ -798,12 +942,124 @@ int raster_ewa_bwd(uint32_t cap, const GaussRec *recs, uint32_t W, uint32_t H, c
     fill_ewa(p, cap, W, H, recs, tile_offsets, flatten_ids);
     {
         ProfScope ps("ewa_blend_bwd", s);
-        launch_bwd_kernel<false, true>(p, alpha, last_ids, grad_image, grad_alpha, moments, s);
+        launch_bwd_kernel<false, true>(p, Chan3{nullptr, 0u}, alpha, last_ids, grad_image, grad_alpha, moments, s);
     }
     GSB_LAUNCH_CHECK();
     return GSB_OK;
 }
 
+} // namespace gsb
+
+namespace gsb {
+// Operator path at NC channels: colors [N,NC], backgrounds [NC], renders [H,W,NC], v_colors [N,NC].  The callers have
+// checked the camera and the channel count; NC != 3 never reaches a rolling shutter.
+template <int NC>
+static int raster_fwd_nc(uint32_t C, uint32_t N, uint64_t n_isects, const float *means, const float *quats,
+                         const float *scales, const float *colors, const float *opacities, const float *backgrounds,
+                         const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size,
+                         const GsbCamera *cam, const int32_t *tile_offsets, const int32_t *flatten_ids, float *renders,
+                         float *alphas, int32_t *last_ids, void *workspace, size_t workspace_bytes, cudaStream_t s) {
+    if (image_width == 0 || image_height == 0) return GSB_OK;
+    if (C != 1) return GSB_E_UNSUPPORTED;       // the reference's kernels are single-camera too (Fwd.cu:197-200)
+    if (tile_size != 16) return GSB_E_UNSUPPORTED; // the reference's callers hard-code 16 (rasterizer.cpp:180)
+    if (!renders || !alphas || !last_ids || !tile_offsets) return GSB_E_INVALID;
+    if (n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids)) return GSB_E_INVALID;
+    if (n_isects > 0x7fffffffull) return GSB_E_INVALID;
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_fwd_workspace(N))
+        return GSB_E_WORKSPACE;
+    if (NC == 3 && rolling_shutter(cam))
+        return raster_rs_fwd(N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
+                             image_height, cam, tile_offsets, flatten_ids, renders, alphas, last_ids, workspace, s);
+    GaussRec *recs = reinterpret_cast<GaussRec *>(workspace);
+    if (N > 0 && n_isects > 0) {
+        {
+            ProfScope ps("raster_prep", s);
+            if constexpr (NC == 3)
+                prep_records_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                    N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, nullptr);
+            else
+                prep_records_nc_kernel<NC><<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                    N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, nullptr);
+        }
+        GSB_LAUNCH_CHECK();
+    }
+    TileParams p;
+    fill_tiles(p, n_isects, (uint32_t)n_isects, 0, image_width, image_height, recs, backgrounds, masks, tile_offsets,
+               flatten_ids, cam);
+    return launch_fwd<NC>(p, cam, Chan3{colors ? colors + 3 : nullptr, (uint32_t)NC}, renders, alphas, last_ids, s);
+}
+
+template <int NC>
+static int raster_bwd_nc(uint32_t C, uint32_t N, uint64_t n_isects, const float *means, const float *quats,
+                         const float *scales, const float *colors, const float *opacities, const float *backgrounds,
+                         const uint8_t *masks, uint32_t image_width, uint32_t image_height, uint32_t tile_size,
+                         const GsbCamera *cam, const int32_t *tile_offsets, const int32_t *flatten_ids,
+                         const float *render_alphas, const int32_t *last_ids, const float *v_render_colors,
+                         const float *v_render_alphas, float *v_means, float *v_quats, float *v_scales,
+                         float *v_colors, float *v_opacities, void *workspace, size_t workspace_bytes, cudaStream_t s) {
+    if (N == 0) return GSB_OK;
+    if (C != 1) return GSB_E_UNSUPPORTED;
+    if (tile_size != 16) return GSB_E_UNSUPPORTED;
+    if (!v_means || !v_quats || !v_scales || !v_colors || !v_opacities) return GSB_E_INVALID;
+    if (n_isects == 0 || image_width == 0 || image_height == 0) { // Bwd.cu:434-437: gradients stay zero
+        GSB_CUDA_TRY(cudaMemsetAsync(v_means, 0, (size_t)N * 12, s));
+        GSB_CUDA_TRY(cudaMemsetAsync(v_quats, 0, (size_t)N * 16, s));
+        GSB_CUDA_TRY(cudaMemsetAsync(v_scales, 0, (size_t)N * 12, s));
+        GSB_CUDA_TRY(cudaMemsetAsync(v_colors, 0, (size_t)N * 4 * NC, s));
+        GSB_CUDA_TRY(cudaMemsetAsync(v_opacities, 0, (size_t)N * 4, s));
+        return GSB_OK;
+    }
+    if (!means || !quats || !scales || !colors || !opacities || !flatten_ids || !tile_offsets || !render_alphas ||
+        !last_ids || !v_render_colors || !v_render_alphas)
+        return GSB_E_INVALID;
+    if (n_isects > 0x7fffffffull) return GSB_E_INVALID;
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_bwd_workspace(N))
+        return GSB_E_WORKSPACE;
+    if (NC == 3 && rolling_shutter(cam))
+        return raster_rs_bwd(N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
+                             image_height, cam, tile_offsets, flatten_ids, render_alphas, last_ids, v_render_colors,
+                             v_render_alphas, v_means, v_quats, v_scales, v_colors, v_opacities, workspace,
+                             align256((size_t)N * sizeof(GaussRec)), s);
+    GaussRec *recs = reinterpret_cast<GaussRec *>(workspace);
+    float *moments = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align256((size_t)N * sizeof(GaussRec)));
+    {
+        ProfScope ps("raster_prep", s);
+        if constexpr (NC == 3)
+            prep_records_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, moments);
+        else
+            prep_records_nc_kernel<NC><<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, moments);
+    }
+    GSB_LAUNCH_CHECK();
+    TileParams p;
+    fill_tiles(p, n_isects, (uint32_t)n_isects, 0, image_width, image_height, recs, backgrounds, masks, tile_offsets,
+               flatten_ids, cam);
+    if (int rc = launch_bwd<NC>(p, cam, Chan3{colors + 3, (uint32_t)NC}, render_alphas, last_ids, v_render_colors,
+                                v_render_alphas, moments, s))
+        return rc;
+    {
+        ProfScope ps("raster_finalize", s);
+        if constexpr (NC == 3)
+            finalize_grads_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                N, means, quats, scales, opacities, cam->viewmats0, cam->Ks, recs, moments, v_means, v_quats, v_scales,
+                v_colors, v_opacities);
+        else
+            finalize_grads_nc_kernel<NC><<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
+                N, means, quats, scales, opacities, cam->viewmats0, cam->Ks, recs, moments, v_means, v_quats, v_scales,
+                v_colors, v_opacities);
+    }
+    GSB_LAUNCH_CHECK();
+    return GSB_OK;
+}
+
+// Channel count and rolling shutter of the *_nc / *_recs_nc entry points, checked before anything else.
+static int check_channels(uint32_t channels, const GsbCamera *cam) {
+    if (channels != 1 && channels != 3 && channels != 4) return GSB_E_UNSUPPORTED;
+    if (int rc = check_camera(cam)) return rc;
+    if (channels != 3 && rolling_shutter(cam)) return GSB_E_UNSUPPORTED; // gsb_raster_rs.cu blends three channels
+    return GSB_OK;
+}
 } // namespace gsb
 
 extern "C" int gsb_raster_fwd(uint32_t C, uint32_t N, uint64_t n_isects, const float *means, const float *quats,
@@ -814,31 +1070,30 @@ extern "C" int gsb_raster_fwd(uint32_t C, uint32_t N, uint64_t n_isects, const f
                               int32_t *last_ids, void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
     using namespace gsb;
     if (int rc = check_camera(cam)) return rc;
-    if (image_width == 0 || image_height == 0) return GSB_OK;
-    if (C != 1) return GSB_E_UNSUPPORTED;       // the reference's kernels are single-camera too (Fwd.cu:197-200)
-    if (tile_size != 16) return GSB_E_UNSUPPORTED; // the reference's callers hard-code 16 (rasterizer.cpp:180)
-    if (!renders || !alphas || !last_ids || !tile_offsets) return GSB_E_INVALID;
-    if (n_isects > 0 && (!means || !quats || !scales || !colors || !opacities || !flatten_ids)) return GSB_E_INVALID;
-    if (n_isects > 0x7fffffffull) return GSB_E_INVALID;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_fwd_workspace(N))
-        return GSB_E_WORKSPACE;
+    return raster_fwd_nc<3>(C, N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
+                            image_height, tile_size, cam, tile_offsets, flatten_ids, renders, alphas, last_ids,
+                            workspace, workspace_bytes, as_stream(stream));
+}
+
+extern "C" int gsb_raster_fwd_nc(uint32_t C, uint32_t N, uint64_t n_isects, uint32_t channels, const float *means,
+                                 const float *quats, const float *scales, const float *colors, const float *opacities,
+                                 const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+                                 uint32_t image_height, uint32_t tile_size, const GsbCamera *cam,
+                                 const int32_t *tile_offsets, const int32_t *flatten_ids, float *renders,
+                                 float *alphas, int32_t *last_ids, void *workspace, size_t workspace_bytes,
+                                 gsb_stream_t stream) {
+    using namespace gsb;
+    if (int rc = check_channels(channels, cam)) return rc;
     cudaStream_t s = as_stream(stream);
-    if (rolling_shutter(cam))
-        return raster_rs_fwd(N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
-                             image_height, cam, tile_offsets, flatten_ids, renders, alphas, last_ids, workspace, s);
-    GaussRec *recs = reinterpret_cast<GaussRec *>(workspace);
-    if (N > 0 && n_isects > 0) {
-        {
-            ProfScope ps("raster_prep", s);
-            prep_records_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
-                N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, nullptr);
-        }
-        GSB_LAUNCH_CHECK();
+#define GSB_RASTER_FWD_ARGS                                                                                            \
+    C, N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width, image_height, tile_size, \
+        cam, tile_offsets, flatten_ids, renders, alphas, last_ids, workspace, workspace_bytes, s
+    switch (channels) {
+        case 1: return raster_fwd_nc<1>(GSB_RASTER_FWD_ARGS);
+        case 4: return raster_fwd_nc<4>(GSB_RASTER_FWD_ARGS);
+        default: return raster_fwd_nc<3>(GSB_RASTER_FWD_ARGS);
     }
-    TileParams p;
-    fill_tiles(p, n_isects, (uint32_t)n_isects, 0, image_width, image_height, recs, backgrounds, masks, tile_offsets,
-               flatten_ids, cam);
-    return launch_fwd(p, cam, renders, alphas, last_ids, s);
+#undef GSB_RASTER_FWD_ARGS
 }
 
 extern "C" int gsb_raster_bwd(uint32_t C, uint32_t N, uint64_t n_isects, const float *means, const float *quats,
@@ -851,56 +1106,74 @@ extern "C" int gsb_raster_bwd(uint32_t C, uint32_t N, uint64_t n_isects, const f
                               void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
     using namespace gsb;
     if (int rc = check_camera(cam)) return rc;
-    if (N == 0) return GSB_OK;
-    if (C != 1) return GSB_E_UNSUPPORTED;
-    if (tile_size != 16) return GSB_E_UNSUPPORTED;
-    if (!v_means || !v_quats || !v_scales || !v_colors || !v_opacities) return GSB_E_INVALID;
+    return raster_bwd_nc<3>(C, N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
+                            image_height, tile_size, cam, tile_offsets, flatten_ids, render_alphas, last_ids,
+                            v_render_colors, v_render_alphas, v_means, v_quats, v_scales, v_colors, v_opacities,
+                            workspace, workspace_bytes, as_stream(stream));
+}
+
+extern "C" int gsb_raster_bwd_nc(uint32_t C, uint32_t N, uint64_t n_isects, uint32_t channels, const float *means,
+                                 const float *quats, const float *scales, const float *colors, const float *opacities,
+                                 const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+                                 uint32_t image_height, uint32_t tile_size, const GsbCamera *cam,
+                                 const int32_t *tile_offsets, const int32_t *flatten_ids, const float *render_alphas,
+                                 const int32_t *last_ids, const float *v_render_colors, const float *v_render_alphas,
+                                 float *v_means, float *v_quats, float *v_scales, float *v_colors, float *v_opacities,
+                                 void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int rc = check_channels(channels, cam)) return rc;
     cudaStream_t s = as_stream(stream);
-    if (n_isects == 0 || image_width == 0 || image_height == 0) { // Bwd.cu:434-437: gradients stay zero
-        GSB_CUDA_TRY(cudaMemsetAsync(v_means, 0, (size_t)N * 12, s));
-        GSB_CUDA_TRY(cudaMemsetAsync(v_quats, 0, (size_t)N * 16, s));
-        GSB_CUDA_TRY(cudaMemsetAsync(v_scales, 0, (size_t)N * 12, s));
-        GSB_CUDA_TRY(cudaMemsetAsync(v_colors, 0, (size_t)N * 12, s));
-        GSB_CUDA_TRY(cudaMemsetAsync(v_opacities, 0, (size_t)N * 4, s));
-        return GSB_OK;
+#define GSB_RASTER_BWD_ARGS                                                                                            \
+    C, N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width, image_height, tile_size, \
+        cam, tile_offsets, flatten_ids, render_alphas, last_ids, v_render_colors, v_render_alphas, v_means, v_quats,   \
+        v_scales, v_colors, v_opacities, workspace, workspace_bytes, s
+    switch (channels) {
+        case 1: return raster_bwd_nc<1>(GSB_RASTER_BWD_ARGS);
+        case 4: return raster_bwd_nc<4>(GSB_RASTER_BWD_ARGS);
+        default: return raster_bwd_nc<3>(GSB_RASTER_BWD_ARGS);
     }
-    if (!means || !quats || !scales || !colors || !opacities || !flatten_ids || !tile_offsets || !render_alphas ||
-        !last_ids || !v_render_colors || !v_render_alphas)
-        return GSB_E_INVALID;
-    if (n_isects > 0x7fffffffull) return GSB_E_INVALID;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_bwd_workspace(N))
-        return GSB_E_WORKSPACE;
-    if (rolling_shutter(cam))
-        return raster_rs_bwd(N, n_isects, means, quats, scales, colors, opacities, backgrounds, masks, image_width,
-                             image_height, cam, tile_offsets, flatten_ids, render_alphas, last_ids, v_render_colors,
-                             v_render_alphas, v_means, v_quats, v_scales, v_colors, v_opacities, workspace,
-                             align256((size_t)N * sizeof(GaussRec)), s);
-    GaussRec *recs = reinterpret_cast<GaussRec *>(workspace);
-    float *moments = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align256((size_t)N * sizeof(GaussRec)));
-    {
-        ProfScope ps("raster_prep", s);
-        prep_records_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
-            N, means, quats, scales, colors, opacities, cam->viewmats0, cam->Ks, recs, moments);
-    }
-    GSB_LAUNCH_CHECK();
-    TileParams p;
-    fill_tiles(p, n_isects, (uint32_t)n_isects, 0, image_width, image_height, recs, backgrounds, masks, tile_offsets,
-               flatten_ids, cam);
-    if (int rc = launch_bwd(p, cam, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, s)) return rc;
-    {
-        ProfScope ps("raster_finalize", s);
-        finalize_grads_kernel<<<(N + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, s>>>(
-            N, means, quats, scales, opacities, cam->viewmats0, cam->Ks, recs, moments, v_means, v_quats, v_scales,
-            v_colors, v_opacities);
-    }
-    GSB_LAUNCH_CHECK();
-    return GSB_OK;
+#undef GSB_RASTER_BWD_ARGS
 }
 
 // ---- fused path (SURVEY.md 8f1): blend forward / backward on records made by gsb_fused_front ---------------------------
 // `workspace` is the fused workspace ([records][moments], gsb_fused_workspace); tile_offsets has th*tw + 1 entries
 // (gsb_isect_plan with tile_offsets_total), so no host-side intersection count is needed: `capacity` is only the size
 // of flatten_ids.
+namespace gsb {
+static int check_recs(uint32_t N, uint32_t capacity, const void *workspace, size_t workspace_bytes,
+                      const int32_t *flatten_ids) {
+    if (capacity > 0 && !flatten_ids) return GSB_E_INVALID;
+    if (capacity > 0x7fffffffu) return GSB_E_INVALID;
+    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_bwd_workspace(N))
+        return GSB_E_WORKSPACE;
+    return GSB_OK;
+}
+template <int NC>
+static int raster_fwd_recs(uint32_t N, uint32_t capacity, const void *workspace, size_t workspace_bytes,
+                           const float *depths, const float *backgrounds, const uint8_t *masks, uint32_t image_width,
+                           uint32_t image_height, const GsbCamera *cam, const int32_t *tile_offsets,
+                           const int32_t *flatten_ids, float *renders, float *alphas, int32_t *last_ids,
+                           cudaStream_t s) {
+    TileParams p;
+    fill_tiles(p, 0, capacity, 1, image_width, image_height, reinterpret_cast<const GaussRec *>(workspace), backgrounds,
+               masks, tile_offsets, flatten_ids, cam);
+    return launch_fwd<NC>(p, cam, Chan3{depths, 1u}, renders, alphas, last_ids, s);
+}
+template <int NC>
+static int raster_bwd_recs(uint32_t N, uint32_t capacity, void *workspace, const float *depths,
+                           const float *backgrounds, const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+                           const GsbCamera *cam, const int32_t *tile_offsets, const int32_t *flatten_ids,
+                           const float *render_alphas, const int32_t *last_ids, const float *v_render_colors,
+                           const float *v_render_alphas, cudaStream_t s) {
+    float *moments = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align256((size_t)N * sizeof(GaussRec)));
+    TileParams p;
+    fill_tiles(p, 0, capacity, 1, image_width, image_height, reinterpret_cast<const GaussRec *>(workspace), backgrounds,
+               masks, tile_offsets, flatten_ids, cam);
+    return launch_bwd<NC>(p, cam, Chan3{depths, 1u}, render_alphas, last_ids, v_render_colors, v_render_alphas, moments,
+                          s);
+}
+} // namespace gsb
+
 extern "C" int gsb_raster_fwd_recs(uint32_t N, uint32_t capacity, const void *workspace, size_t workspace_bytes,
                                    const float *backgrounds, const uint8_t *masks, uint32_t image_width,
                                    uint32_t image_height, const GsbCamera *cam, const int32_t *tile_offsets,
@@ -911,14 +1184,33 @@ extern "C" int gsb_raster_fwd_recs(uint32_t N, uint32_t capacity, const void *wo
     if (rolling_shutter(cam)) return GSB_E_UNSUPPORTED; // the fused path is global-shutter only
     if (image_width == 0 || image_height == 0) return GSB_OK;
     if (!renders || !alphas || !last_ids || !tile_offsets) return GSB_E_INVALID;
-    if (capacity > 0 && !flatten_ids) return GSB_E_INVALID;
-    if (capacity > 0x7fffffffu) return GSB_E_INVALID;
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_bwd_workspace(N))
-        return GSB_E_WORKSPACE;
-    TileParams p;
-    fill_tiles(p, 0, capacity, 1, image_width, image_height, reinterpret_cast<const GaussRec *>(workspace), backgrounds,
-               masks, tile_offsets, flatten_ids, cam);
-    return launch_fwd(p, cam, renders, alphas, last_ids, as_stream(stream));
+    if (int rc = check_recs(N, capacity, workspace, workspace_bytes, flatten_ids)) return rc;
+    return raster_fwd_recs<3>(N, capacity, workspace, workspace_bytes, nullptr, backgrounds, masks, image_width,
+                              image_height, cam, tile_offsets, flatten_ids, renders, alphas, last_ids, as_stream(stream));
+}
+
+extern "C" int gsb_raster_fwd_recs_nc(uint32_t N, uint32_t capacity, uint32_t channels, const void *workspace,
+                                      size_t workspace_bytes, const float *depths, const float *backgrounds,
+                                      const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+                                      const GsbCamera *cam, const int32_t *tile_offsets, const int32_t *flatten_ids,
+                                      float *renders, float *alphas, int32_t *last_ids, gsb_stream_t stream) {
+    using namespace gsb;
+    if (int rc = check_channels(channels, cam)) return rc;
+    if (rolling_shutter(cam)) return GSB_E_UNSUPPORTED; // the fused path is global-shutter only
+    if (channels == 4 && N > 0 && !depths) return GSB_E_INVALID;
+    if (image_width == 0 || image_height == 0) return GSB_OK;
+    if (!renders || !alphas || !last_ids || !tile_offsets) return GSB_E_INVALID;
+    if (int rc = check_recs(N, capacity, workspace, workspace_bytes, flatten_ids)) return rc;
+    cudaStream_t s = as_stream(stream);
+#define GSB_RECS_FWD_ARGS                                                                                              \
+    N, capacity, workspace, workspace_bytes, depths, backgrounds, masks, image_width, image_height, cam, tile_offsets, \
+        flatten_ids, renders, alphas, last_ids, s
+    switch (channels) {
+        case 1: return raster_fwd_recs<1>(GSB_RECS_FWD_ARGS);
+        case 4: return raster_fwd_recs<4>(GSB_RECS_FWD_ARGS);
+        default: return raster_fwd_recs<3>(GSB_RECS_FWD_ARGS);
+    }
+#undef GSB_RECS_FWD_ARGS
 }
 
 extern "C" int gsb_raster_bwd_recs(uint32_t N, uint32_t capacity, void *workspace, size_t workspace_bytes,
@@ -931,14 +1223,34 @@ extern "C" int gsb_raster_bwd_recs(uint32_t N, uint32_t capacity, void *workspac
     if (rolling_shutter(cam)) return GSB_E_UNSUPPORTED;
     if (N == 0 || image_width == 0 || image_height == 0) return GSB_OK;
     if (!tile_offsets || !render_alphas || !last_ids || !v_render_colors || !v_render_alphas) return GSB_E_INVALID;
-    if (capacity > 0 && !flatten_ids) return GSB_E_INVALID;
-    if (capacity > 0x7fffffffu) return GSB_E_INVALID;
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < gsb_raster_bwd_workspace(N))
-        return GSB_E_WORKSPACE;
-    float *moments = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align256((size_t)N * sizeof(GaussRec)));
-    TileParams p;
-    fill_tiles(p, 0, capacity, 1, image_width, image_height, reinterpret_cast<const GaussRec *>(workspace), backgrounds,
-               masks, tile_offsets, flatten_ids, cam);
-    return launch_bwd(p, cam, render_alphas, last_ids, v_render_colors, v_render_alphas, moments, as_stream(stream));
+    if (int rc = check_recs(N, capacity, workspace, workspace_bytes, flatten_ids)) return rc;
+    return raster_bwd_recs<3>(N, capacity, workspace, nullptr, backgrounds, masks, image_width, image_height, cam,
+                              tile_offsets, flatten_ids, render_alphas, last_ids, v_render_colors, v_render_alphas,
+                              as_stream(stream));
 }
 
+extern "C" int gsb_raster_bwd_recs_nc(uint32_t N, uint32_t capacity, uint32_t channels, void *workspace,
+                                      size_t workspace_bytes, const float *depths, const float *backgrounds,
+                                      const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+                                      const GsbCamera *cam, const int32_t *tile_offsets, const int32_t *flatten_ids,
+                                      const float *render_alphas, const int32_t *last_ids,
+                                      const float *v_render_colors, const float *v_render_alphas,
+                                      gsb_stream_t stream) {
+    using namespace gsb;
+    if (int rc = check_channels(channels, cam)) return rc;
+    if (rolling_shutter(cam)) return GSB_E_UNSUPPORTED;
+    if (channels == 4 && N > 0 && !depths) return GSB_E_INVALID;
+    if (N == 0 || image_width == 0 || image_height == 0) return GSB_OK;
+    if (!tile_offsets || !render_alphas || !last_ids || !v_render_colors || !v_render_alphas) return GSB_E_INVALID;
+    if (int rc = check_recs(N, capacity, workspace, workspace_bytes, flatten_ids)) return rc;
+    cudaStream_t s = as_stream(stream);
+#define GSB_RECS_BWD_ARGS                                                                                              \
+    N, capacity, workspace, depths, backgrounds, masks, image_width, image_height, cam, tile_offsets, flatten_ids,     \
+        render_alphas, last_ids, v_render_colors, v_render_alphas, s
+    switch (channels) {
+        case 1: return raster_bwd_recs<1>(GSB_RECS_BWD_ARGS);
+        case 4: return raster_bwd_recs<4>(GSB_RECS_BWD_ARGS);
+        default: return raster_bwd_recs<3>(GSB_RECS_BWD_ARGS);
+    }
+#undef GSB_RECS_BWD_ARGS
+}

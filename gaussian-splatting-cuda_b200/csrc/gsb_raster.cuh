@@ -213,6 +213,9 @@ enum MomentSlot : int {
     kS_G = 0, kS_W1X = 1, kS_W1Y = 2, kS_W1XX = 3, kS_W1XY = 4, kS_W1YY = 5, kS_CR = 6, kS_CB = 7,
     kS_W2 = 8, kS_W2X = 9, kS_W2Y = 10, kS_W2XX = 11, kS_W2XY = 12, kS_W2YY = 13, kS_CG = 14, kS_PAD = 15
 };
+// Channel counts of the blend (render modes, DESIGN.md 4.16): 3 = RGB, 1 = depth only (colour slot kS_CR), 4 = RGB +
+// depth.  The fourth channel's gradient takes the pad slot, the partner of kS_CB in the butterfly's first stage.
+constexpr int kS_C4 = kS_PAD;
 
 // chain-rule arithmetic type of the finalize step (float: validated against the f64 oracle by the parity tests)
 typedef float FT;

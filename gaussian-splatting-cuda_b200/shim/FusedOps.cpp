@@ -109,6 +109,19 @@ Cam make_cam(const at::Tensor &viewmat, const at::Tensor &K, gsplat::CameraModel
 
 namespace gsplat {
 
+namespace {
+uint32_t mode_channels(RenderMode m) {
+    switch (m) {
+        case RenderMode::RGB: return 3;
+        case RenderMode::D:
+        case RenderMode::ED: return 1;
+        case RenderMode::RGB_D:
+        case RenderMode::RGB_ED: return 4;
+    }
+    TORCH_CHECK(false, "fused rasterizer: invalid render mode ", static_cast<int>(m));
+}
+} // namespace
+
 GSB_EXPORT FusedForwardResult rasterize_from_world_fused_fwd(
     const at::Tensor means, const at::Tensor sh0, const at::Tensor shN, const at::Tensor scaling_raw,
     const at::Tensor rotation_raw, const at::Tensor opacity_raw, const uint32_t sh_degree, const float scaling_modifier,
@@ -118,6 +131,26 @@ GSB_EXPORT FusedForwardResult rasterize_from_world_fused_fwd(
     const UnscentedTransformParameters ut_params, const at::optional<at::Tensor> radial_coeffs,
     const at::optional<at::Tensor> tangential_coeffs, const at::optional<at::Tensor> thin_prism_coeffs,
     const int64_t isect_capacity, const bool prepare_backward) {
+    return rasterize_from_world_fused_fwd(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree,
+                                          scaling_modifier, viewmat, K, image_width, image_height, eps2d, near_plane,
+                                          far_plane, radius_clip, backgrounds, camera_model, ut_params, radial_coeffs,
+                                          tangential_coeffs, thin_prism_coeffs, isect_capacity, prepare_backward,
+                                          RenderMode::RGB);
+}
+
+GSB_EXPORT FusedForwardResult rasterize_from_world_fused_fwd(
+    const at::Tensor means, const at::Tensor sh0, const at::Tensor shN, const at::Tensor scaling_raw,
+    const at::Tensor rotation_raw, const at::Tensor opacity_raw, const uint32_t sh_degree, const float scaling_modifier,
+    const at::Tensor viewmat, const at::Tensor K, const uint32_t image_width, const uint32_t image_height,
+    const float eps2d, const float near_plane, const float far_plane, const float radius_clip,
+    const at::optional<at::Tensor> backgrounds, const CameraModelType camera_model,
+    const UnscentedTransformParameters ut_params, const at::optional<at::Tensor> radial_coeffs,
+    const at::optional<at::Tensor> tangential_coeffs, const at::optional<at::Tensor> thin_prism_coeffs,
+    const int64_t isect_capacity, const bool prepare_backward, const RenderMode render_mode) {
+    const uint32_t channels = mode_channels(render_mode);
+    TORCH_CHECK(render_mode == RenderMode::RGB || !backgrounds.has_value() || !backgrounds->defined() ||
+                    backgrounds->numel() == 0 || backgrounds->numel() == channels,
+                "fused rasterizer: backgrounds must be [1,", channels, "] in this render mode");
     const c10::cuda::CUDAGuard guard(means.device());
     Splats sp = make_splats(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree, scaling_modifier);
     Cam cam = make_cam(viewmat, K, camera_model, ut_params, radial_coeffs, tangential_coeffs, thin_prism_coeffs);
@@ -131,9 +164,10 @@ GSB_EXPORT FusedForwardResult rasterize_from_world_fused_fwd(
     r.depths = at::empty({1, N}, f32);
     const size_t ws_bytes = gsb_fused_workspace(N);
     r.workspace = at::empty({(int64_t)ws_bytes}, means.options().dtype(at::kByte));
-    gsb_check(gsb_fused_front(&sp.raw, &cam.cam, image_width, image_height, eps2d, near_plane, far_plane, radius_clip,
-                              prepare_backward ? 1 : 0, r.radii.data_ptr<int32_t>(), r.means2d.data_ptr<float>(),
-                              r.depths.data_ptr<float>(), r.workspace.data_ptr(), ws_bytes, cur_stream()),
+    gsb_check(gsb_fused_front_mode(&sp.raw, &cam.cam, image_width, image_height, eps2d, near_plane, far_plane,
+                                   radius_clip, prepare_backward ? 1 : 0, static_cast<int>(render_mode),
+                                   r.radii.data_ptr<int32_t>(), r.means2d.data_ptr<float>(), r.depths.data_ptr<float>(),
+                                   r.workspace.data_ptr(), ws_bytes, cur_stream()),
               "rasterize_from_world_fused_fwd/front");
 
     // intersect: plan (everything that needs no host-side count), then the direct placement
@@ -157,13 +191,14 @@ GSB_EXPORT FusedForwardResult rasterize_from_world_fused_fwd(
                                          r.flatten_ids.data_ptr<int32_t>(), cur_stream()),
                   "rasterize_from_world_fused_fwd/emit");
     }
-    r.renders = at::empty({1, image_height, image_width, 3}, f32);
+    r.renders = at::empty({1, image_height, image_width, channels}, f32);
     r.alphas = at::empty({1, image_height, image_width, 1}, f32);
     r.last_ids = at::empty({1, image_height, image_width}, i32);
-    gsb_check(gsb_raster_fwd_recs(N, (uint32_t)capacity, r.workspace.data_ptr(), ws_bytes, opt_f32(backgrounds), nullptr,
-                                  image_width, image_height, &cam.cam, r.tile_offsets.data_ptr<int32_t>(),
-                                  capacity ? r.flatten_ids.data_ptr<int32_t>() : nullptr, r.renders.data_ptr<float>(),
-                                  r.alphas.data_ptr<float>(), r.last_ids.data_ptr<int32_t>(), cur_stream()),
+    gsb_check(gsb_raster_fwd_recs_nc(N, (uint32_t)capacity, channels, r.workspace.data_ptr(), ws_bytes,
+                                     r.depths.data_ptr<float>(), opt_f32(backgrounds), nullptr, image_width,
+                                     image_height, &cam.cam, r.tile_offsets.data_ptr<int32_t>(),
+                                     capacity ? r.flatten_ids.data_ptr<int32_t>() : nullptr, r.renders.data_ptr<float>(),
+                                     r.alphas.data_ptr<float>(), r.last_ids.data_ptr<int32_t>(), cur_stream()),
               "rasterize_from_world_fused_fwd/blend");
     return r;
 }
@@ -181,6 +216,31 @@ rasterize_from_world_fused_bwd(const at::Tensor means, const at::Tensor sh0, con
                                const at::Tensor tile_offsets, const at::Tensor flatten_ids, at::Tensor workspace,
                                const at::Tensor render_alphas, const at::Tensor last_ids,
                                const at::Tensor v_render_colors, const at::Tensor v_render_alphas) {
+    return rasterize_from_world_fused_bwd(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree,
+                                          scaling_modifier, viewmat, K, image_width, image_height, backgrounds,
+                                          camera_model, ut_params, radial_coeffs, tangential_coeffs, thin_prism_coeffs,
+                                          radii, tile_offsets, flatten_ids, workspace, render_alphas, last_ids,
+                                          v_render_colors, v_render_alphas, at::Tensor(), RenderMode::RGB);
+}
+
+GSB_EXPORT std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor>
+rasterize_from_world_fused_bwd(const at::Tensor means, const at::Tensor sh0, const at::Tensor shN,
+                               const at::Tensor scaling_raw, const at::Tensor rotation_raw, const at::Tensor opacity_raw,
+                               const uint32_t sh_degree, const float scaling_modifier, const at::Tensor viewmat,
+                               const at::Tensor K, const uint32_t image_width, const uint32_t image_height,
+                               const at::optional<at::Tensor> backgrounds, const CameraModelType camera_model,
+                               const UnscentedTransformParameters ut_params,
+                               const at::optional<at::Tensor> radial_coeffs,
+                               const at::optional<at::Tensor> tangential_coeffs,
+                               const at::optional<at::Tensor> thin_prism_coeffs, const at::Tensor radii,
+                               const at::Tensor tile_offsets, const at::Tensor flatten_ids, at::Tensor workspace,
+                               const at::Tensor render_alphas, const at::Tensor last_ids,
+                               const at::Tensor v_render_colors, const at::Tensor v_render_alphas,
+                               const at::Tensor depths, const RenderMode render_mode) {
+    const uint32_t channels = mode_channels(render_mode);
+    TORCH_CHECK(render_mode == RenderMode::RGB || !backgrounds.has_value() || !backgrounds->defined() ||
+                    backgrounds->numel() == 0 || backgrounds->numel() == channels,
+                "fused rasterizer: backgrounds must be [1,", channels, "] in this render mode");
     const c10::cuda::CUDAGuard guard(means.device());
     Splats sp = make_splats(means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, sh_degree, scaling_modifier);
     Cam cam = make_cam(viewmat, K, camera_model, ut_params, radial_coeffs, tangential_coeffs, thin_prism_coeffs);
@@ -193,17 +253,26 @@ rasterize_from_world_fused_bwd(const at::Tensor means, const at::Tensor sh0, con
     const uint32_t N = sp.raw.N;
     const size_t ws_bytes = (size_t)workspace.numel();
     const int64_t capacity = flatten_ids.numel();
-    gsb_check(gsb_raster_bwd_recs(N, (uint32_t)capacity, workspace.data_ptr(), ws_bytes, opt_f32(backgrounds), nullptr,
-                                  image_width, image_height, &cam.cam, tile_offsets.data_ptr<int32_t>(),
-                                  capacity ? flatten_ids.data_ptr<int32_t>() : nullptr, render_alphas.data_ptr<float>(),
-                                  last_ids.data_ptr<int32_t>(), v_render_colors.data_ptr<float>(),
-                                  v_render_alphas.data_ptr<float>(), cur_stream()),
+    TORCH_CHECK(v_render_colors.numel() == (int64_t)image_width * image_height * channels,
+                "fused backward: v_render_colors must be [1,H,W,", channels, "]");
+    // RGB_D / RGB_ED: the blend reads the fourth channel from the forward's depths, by the record's Gaussian index
+    if (channels == 4) {
+        CHECK_F32(depths);
+        TORCH_CHECK(depths.numel() == (int64_t)N, "fused backward: depths must be the forward's [1,N] depths");
+    }
+    gsb_check(gsb_raster_bwd_recs_nc(N, (uint32_t)capacity, channels, workspace.data_ptr(), ws_bytes,
+                                     channels == 4 ? depths.data_ptr<float>() : nullptr, opt_f32(backgrounds), nullptr,
+                                     image_width, image_height, &cam.cam, tile_offsets.data_ptr<int32_t>(),
+                                     capacity ? flatten_ids.data_ptr<int32_t>() : nullptr,
+                                     render_alphas.data_ptr<float>(), last_ids.data_ptr<int32_t>(),
+                                     v_render_colors.data_ptr<float>(), v_render_alphas.data_ptr<float>(),
+                                     cur_stream()),
               "rasterize_from_world_fused_bwd/blend");
     at::Tensor v_means = at::empty_like(means), v_sh0 = at::empty_like(sh0), v_scaling = at::empty_like(scaling_raw);
     at::Tensor v_rotation = at::empty_like(rotation_raw), v_opacity = at::empty_like(opacity_raw);
     at::Tensor v_shN = shN.defined() ? at::empty_like(shN) : at::Tensor();
-    gsb_check(gsb_fused_back(&sp.raw, &cam.cam, image_width, image_height, radii.data_ptr<int32_t>(), workspace.data_ptr(),
-                             ws_bytes, v_means.data_ptr<float>(), v_sh0.data_ptr<float>(),
+    gsb_check(gsb_fused_back_mode(&sp.raw, &cam.cam, image_width, image_height, static_cast<int>(render_mode),
+                                  radii.data_ptr<int32_t>(), workspace.data_ptr(), ws_bytes, v_means.data_ptr<float>(), v_sh0.data_ptr<float>(),
                              (v_shN.defined() && v_shN.numel()) ? v_shN.data_ptr<float>() : nullptr,
                              v_scaling.data_ptr<float>(), v_rotation.data_ptr<float>(), v_opacity.data_ptr<float>(),
                              cur_stream()),

@@ -325,8 +325,10 @@ GSB_EXPORT std::tuple<at::Tensor, at::Tensor, at::Tensor> rasterize_to_pixels_fr
     const uint32_t C = tile_offsets.size(0);
     const uint32_t N = means.size(0);
     const uint32_t channels = colors.size(-1);
-    TORCH_CHECK(channels == 3, "Unsupported number of channels: ", channels,
-                " (only RGB is reachable in the reference, Rasterization.cpp:65)");
+    // 3 = RGB; 1 and 4 are the depth render modes (D / ED, RGB_D / RGB_ED: rasterizer.cpp:272-298)
+    TORCH_CHECK(channels == 1 || channels == 3 || channels == 4, "Unsupported number of channels: ", channels);
+    TORCH_CHECK(channels == 3 || !backgrounds.has_value() || backgrounds->numel() == (int64_t)C * channels,
+                "backgrounds must be [C, ", channels, "]");
     at::Tensor renders = at::empty({C, image_height, image_width, channels}, means.options());
     at::Tensor alphas = at::empty({C, image_height, image_width, 1}, means.options());
     at::Tensor last_ids = at::empty({C, image_height, image_width}, means.options().dtype(at::kInt));
@@ -334,7 +336,7 @@ GSB_EXPORT std::tuple<at::Tensor, at::Tensor, at::Tensor> rasterize_to_pixels_fr
                                 tangential_coeffs, thin_prism_coeffs);
     const size_t ws_bytes = gsb_raster_fwd_workspace(N);
     at::Tensor ws = byte_workspace(ws_bytes, means);
-    gsb_check(gsb_raster_fwd(C, N, (uint64_t)flatten_ids.size(0), means.data_ptr<float>(), quats.data_ptr<float>(),
+    gsb_check(gsb_raster_fwd_nc(C, N, (uint64_t)flatten_ids.size(0), channels, means.data_ptr<float>(), quats.data_ptr<float>(),
                              scales.data_ptr<float>(), colors.data_ptr<float>(), opacities.data_ptr<float>(),
                              opt_f32(backgrounds),
                              masks.has_value() ? reinterpret_cast<const uint8_t *>(masks->data_ptr<bool>()) : nullptr,
@@ -377,7 +379,9 @@ rasterize_to_pixels_from_world_3dgs_bwd(
     const uint32_t C = tile_offsets.size(0);
     const uint32_t N = means.size(0);
     const uint32_t channels = colors.size(-1);
-    TORCH_CHECK(channels == 3, "Unsupported number of channels: ", channels);
+    TORCH_CHECK(channels == 1 || channels == 3 || channels == 4, "Unsupported number of channels: ", channels);
+    TORCH_CHECK(channels == 3 || !backgrounds.has_value() || backgrounds->numel() == (int64_t)C * channels,
+                "backgrounds must be [C, ", channels, "]");
     // every element is written by the backend: no five zero-fills as in Rasterization.cpp:190-194
     at::Tensor v_means = at::empty_like(means);
     at::Tensor v_quats = at::empty_like(quats);
@@ -388,7 +392,7 @@ rasterize_to_pixels_from_world_3dgs_bwd(
                                 tangential_coeffs, thin_prism_coeffs);
     const size_t ws_bytes = gsb_raster_bwd_workspace(N);
     at::Tensor ws = byte_workspace(ws_bytes, means);
-    gsb_check(gsb_raster_bwd(C, N, (uint64_t)flatten_ids.size(0), means.data_ptr<float>(), quats.data_ptr<float>(),
+    gsb_check(gsb_raster_bwd_nc(C, N, (uint64_t)flatten_ids.size(0), channels, means.data_ptr<float>(), quats.data_ptr<float>(),
                              scales.data_ptr<float>(), colors.data_ptr<float>(), opacities.data_ptr<float>(),
                              opt_f32(backgrounds),
                              masks.has_value() ? reinterpret_cast<const uint8_t *>(masks->data_ptr<bool>()) : nullptr,

@@ -178,6 +178,41 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> fused_bwd(
     return std::make_tuple(std::get<0>(r), std::get<1>(r), v_shN, std::get<3>(r), std::get<4>(r), std::get<5>(r));
 }
 
+// The RenderMode overloads (render_mode = gsplat::RenderMode as an int)
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> fused_fwd_mode(
+    const Tensor &means, const Tensor &sh0, const Tensor &shN, const Tensor &scaling_raw, const Tensor &rotation_raw,
+    const Tensor &opacity_raw, int64_t sh_degree, double scaling_modifier, const Tensor &viewmat, const Tensor &K,
+    int64_t width, int64_t height, double eps2d, double near_plane, double far_plane, double radius_clip,
+    const OT &backgrounds, int64_t camera_model, const OT &radial, const OT &tangential, const OT &thin_prism,
+    int64_t isect_capacity, bool prepare_backward, int64_t render_mode) {
+    TORCH_CHECK(render_mode >= 0 && render_mode <= 4, "invalid render mode ", render_mode);
+    auto r = gsplat::rasterize_from_world_fused_fwd(
+        means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, (uint32_t)sh_degree, (float)scaling_modifier, viewmat, K,
+        (uint32_t)width, (uint32_t)height, (float)eps2d, (float)near_plane, (float)far_plane, (float)radius_clip,
+        backgrounds, static_cast<gsplat::CameraModelType>(camera_model), UnscentedTransformParameters{}, radial, tangential,
+        thin_prism, isect_capacity, prepare_backward, static_cast<gsplat::RenderMode>(render_mode));
+    return std::make_tuple(r.renders, r.alphas, r.radii, r.means2d, r.depths, r.last_ids, r.tile_offsets, r.flatten_ids,
+                           r.workspace, r.n_isects);
+}
+
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> fused_bwd_mode(
+    const Tensor &means, const Tensor &sh0, const Tensor &shN, const Tensor &scaling_raw, const Tensor &rotation_raw,
+    const Tensor &opacity_raw, int64_t sh_degree, double scaling_modifier, const Tensor &viewmat, const Tensor &K,
+    int64_t width, int64_t height, const OT &backgrounds, int64_t camera_model, const OT &radial, const OT &tangential,
+    const OT &thin_prism, const Tensor &radii, const Tensor &tile_offsets, const Tensor &flatten_ids, Tensor workspace,
+    const Tensor &render_alphas, const Tensor &last_ids, const Tensor &v_render_colors, const Tensor &v_render_alphas,
+    const Tensor &depths, int64_t render_mode) {
+    TORCH_CHECK(render_mode >= 0 && render_mode <= 4, "invalid render mode ", render_mode);
+    auto r = gsplat::rasterize_from_world_fused_bwd(
+        means, sh0, shN, scaling_raw, rotation_raw, opacity_raw, (uint32_t)sh_degree, (float)scaling_modifier, viewmat, K,
+        (uint32_t)width, (uint32_t)height, backgrounds, static_cast<gsplat::CameraModelType>(camera_model),
+        UnscentedTransformParameters{}, radial, tangential, thin_prism, radii, tile_offsets, flatten_ids, workspace,
+        render_alphas, last_ids, v_render_colors, v_render_alphas, depths, static_cast<gsplat::RenderMode>(render_mode));
+    Tensor v_shN = std::get<2>(r);
+    if (!v_shN.defined()) v_shN = at::empty({0}, means.options());
+    return std::make_tuple(std::get<0>(r), std::get<1>(r), v_shN, std::get<3>(r), std::get<4>(r), std::get<5>(r));
+}
+
 std::tuple<Tensor, Tensor> loss_fused(const Tensor &renders, const Tensor &target, double lambda_dssim, bool compute_grad) {
     auto r = gsplat::photometric_loss_fused(renders, target, (float)lambda_dssim, compute_grad);
     Tensor v = std::get<1>(r);
@@ -244,6 +279,14 @@ TORCH_LIBRARY(gsplat_b200, m) {
           "Tensor tile_offsets, Tensor flatten_ids, Tensor(a!) workspace, Tensor render_alphas, Tensor last_ids, "
           "Tensor v_render_colors, Tensor v_render_alphas) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)",
           &fused_bwd);
+    m.def("rasterize_from_world_fused_fwd_mode", &fused_fwd_mode);
+    m.def("rasterize_from_world_fused_bwd_mode(Tensor means, Tensor sh0, Tensor shN, Tensor scaling_raw, "
+          "Tensor rotation_raw, Tensor opacity_raw, int sh_degree, float scaling_modifier, Tensor viewmat, Tensor K, "
+          "int width, int height, Tensor? backgrounds, int camera_model, Tensor? radial, Tensor? tangential, "
+          "Tensor? thin_prism, Tensor radii, Tensor tile_offsets, Tensor flatten_ids, Tensor(a!) workspace, "
+          "Tensor render_alphas, Tensor last_ids, Tensor v_render_colors, Tensor v_render_alphas, Tensor depths, "
+          "int render_mode) -> (Tensor, Tensor, Tensor, Tensor, Tensor, Tensor)",
+          &fused_bwd_mode);
     m.def("photometric_loss_fused", &loss_fused);
     m.def("photometric_loss_fused_unclamped", &loss_fused_unclamped);
     m.def("fused_adam_step(Tensor(a!)[] params, Tensor[] grads, Tensor(b!)[] exp_avg, Tensor(c!)[] exp_avg_sq, float[] lr, "

@@ -247,6 +247,33 @@ GSB_API int gsb_raster_bwd(
     float *v_means, float *v_quats, float *v_scales, float *v_colors, float *v_opacities,
     void *workspace, size_t workspace_bytes, gsb_stream_t stream);
 
+/* ---- a7 / a8 at 1, 3 or 4 channels: the blend of the reference's render modes (rasterizer.cpp:272-298) -----------
+ * The same operators with `channels` colour channels per Gaussian: colors [C,N,channels], backgrounds
+ * [C,channels] or NULL, renders [C,H,W,channels], v_colors [C,N,channels]; everything else as above, and the same
+ * workspaces.  channels = 1 blends the depth alone (RenderMode D / ED), 4 colour + depth (RGB_D / RGB_ED);
+ * channels = 3 is exactly gsb_raster_fwd / gsb_raster_bwd.  Checked before any launch:
+ *   channels not in {1, 3, 4}                          -> GSB_E_UNSUPPORTED
+ *   channels != 3 with a rolling shutter              -> GSB_E_UNSUPPORTED (the rolling-shutter blend is RGB only)
+ *   a NULL camera or argument pointer                  -> GSB_E_INVALID, as for the 3-channel calls. */
+GSB_API int gsb_raster_fwd_nc(
+    uint32_t C, uint32_t N, uint64_t n_isects, uint32_t channels,
+    const float *means, const float *quats, const float *scales, const float *colors,
+    const float *opacities, const float *backgrounds, const uint8_t *masks,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, const GsbCamera *cam,
+    const int32_t *tile_offsets, const int32_t *flatten_ids,
+    float *renders, float *alphas, int32_t *last_ids,
+    void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_raster_bwd_nc(
+    uint32_t C, uint32_t N, uint64_t n_isects, uint32_t channels,
+    const float *means, const float *quats, const float *scales, const float *colors,
+    const float *opacities, const float *backgrounds, const uint8_t *masks,
+    uint32_t image_width, uint32_t image_height, uint32_t tile_size, const GsbCamera *cam,
+    const int32_t *tile_offsets, const int32_t *flatten_ids,
+    const float *render_alphas, const int32_t *last_ids,
+    const float *v_render_colors, const float *v_render_alphas,
+    float *v_means, float *v_quats, float *v_scales, float *v_colors, float *v_opacities,
+    void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+
 /* ---- SURVEY.md 8(f1): the L3 glue folded into the path -- an EXTENDED operator set over the raw SplatData --------
  * The reference's caller activates the parameters and builds SH inputs with ~10 torch kernels around the
  * operators every step (src/core/splat_data.cpp:267-286: exp / sigmoid / normalize / cat(sh0, shN);
@@ -300,6 +327,46 @@ GSB_API int gsb_fused_back(const GsbSplatRaw *splats, const GsbCamera *cam, uint
                            size_t workspace_bytes, float *v_means, float *v_sh0, float *v_shN /*NULL iff K == 1*/,
                            float *v_scaling, float *v_rotation /*16-byte aligned*/, float *v_opacity,
                            gsb_stream_t stream);
+
+/* Render modes on the fused path (gs::training::RenderMode, rasterizer.hpp:25-31; POINT_CLOUD is not a blend).
+ *   gsb_fused_front_mode   RGB / RGB_D / RGB_ED: the records of gsb_fused_front (SH colour); D / ED: the record's
+ *                          one channel is the camera-space depth written to depths[].
+ *   gsb_raster_fwd_recs_nc / gsb_raster_bwd_recs_nc   the blend at `channels` = 1 (D / ED), 3 (RGB) or 4 (RGB_D /
+ *                          RGB_ED: the fourth channel is read from the front's depths [N]; NULL -> GSB_E_INVALID).
+ *                          backgrounds [channels] or NULL, renders / v_render_colors [H,W,channels].
+ *   gsb_fused_back_mode    as gsb_fused_back; the depth channel's gradient is dropped (the depth is not
+ *                          differentiable, Ops.h:67): D / ED give sh0 / shN gradients of zero.
+ * A render_mode outside GSB_RENDER_* or channels outside {1, 3, 4} -> GSB_E_UNSUPPORTED, checked first.  The
+ * mode passed to the front, the blend's channel count and the mode passed to the back must agree. */
+enum GsbRenderMode {
+    GSB_RENDER_RGB = 0,
+    GSB_RENDER_D = 1,     /* accumulated depth */
+    GSB_RENDER_ED = 2,    /* expected depth: accumulated depth / alpha, divided by the caller */
+    GSB_RENDER_RGB_D = 3,
+    GSB_RENDER_RGB_ED = 4
+};
+GSB_API int gsb_fused_front_mode(const GsbSplatRaw *splats, const GsbCamera *cam, uint32_t image_width,
+                                 uint32_t image_height, float eps2d, float near_plane, float far_plane,
+                                 float radius_clip, int zero_moments, int render_mode,
+                                 int32_t *radii /*[N,2]*/, float *means2d /*[N,2]*/, float *depths /*[N]*/,
+                                 void *workspace, size_t workspace_bytes, gsb_stream_t stream);
+GSB_API int gsb_raster_fwd_recs_nc(uint32_t N, uint32_t capacity, uint32_t channels, const void *workspace,
+                                   size_t workspace_bytes, const float *depths /*[N]*/, const float *backgrounds,
+                                   const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+                                   const GsbCamera *cam, const int32_t *tile_offsets /*[th*tw + 1]*/,
+                                   const int32_t *flatten_ids, float *renders, float *alphas, int32_t *last_ids,
+                                   gsb_stream_t stream);
+GSB_API int gsb_raster_bwd_recs_nc(uint32_t N, uint32_t capacity, uint32_t channels, void *workspace,
+                                   size_t workspace_bytes, const float *depths /*[N]*/, const float *backgrounds,
+                                   const uint8_t *masks, uint32_t image_width, uint32_t image_height,
+                                   const GsbCamera *cam, const int32_t *tile_offsets /*[th*tw + 1]*/,
+                                   const int32_t *flatten_ids, const float *render_alphas, const int32_t *last_ids,
+                                   const float *v_render_colors, const float *v_render_alphas, gsb_stream_t stream);
+GSB_API int gsb_fused_back_mode(const GsbSplatRaw *splats, const GsbCamera *cam, uint32_t image_width,
+                                uint32_t image_height, int render_mode, const int32_t *radii, const void *workspace,
+                                size_t workspace_bytes, float *v_means, float *v_sh0,
+                                float *v_shN /*NULL iff K == 1*/, float *v_scaling,
+                                float *v_rotation /*16-byte aligned*/, float *v_opacity, gsb_stream_t stream);
 
 /* ---- SURVEY.md 8(f2): photometric loss of the training step and its gradient, one kernel -------------------------
  * loss = (1 - lambda) * mean|clamp(render,0,1) - target| + lambda * (1 - mean SSIM_valid)

@@ -9,7 +9,8 @@
 //   backward  rasterize_to_pixels_from_world_3dgs_bwd + spherical_harmonics_bwd + the autograd backward of all of
 //             the above, down to the gradients of the raw parameter tensors
 //
-// C == 1 (one camera per call, like the reference's kernels), RGB, tile size 16, global shutter.
+// C == 1 (one camera per call, like the reference's kernels), tile size 16, global shutter; RGB, or a depth render
+// mode through the RenderMode overloads.
 #pragma once
 
 #include <ATen/core/Tensor.h>
@@ -68,6 +69,38 @@ std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tenso
     const at::Tensor radii, const at::Tensor tile_offsets, const at::Tensor flatten_ids, at::Tensor workspace,
     const at::Tensor render_alphas, const at::Tensor last_ids, const at::Tensor v_render_colors,
     const at::Tensor v_render_alphas);
+
+// Render modes (gs::training::RenderMode, rasterizer.hpp:25-31; POINT_CLOUD is not a blend and has no value here).
+enum class RenderMode { RGB = 0, D = 1, ED = 2, RGB_D = 3, RGB_ED = 4 };
+
+// The same two operators in a render mode: the blend runs at 1 channel (D, ED: the camera-space depth), 3 (RGB) or 4
+// (RGB_D, RGB_ED: SH colour + depth).  renders / v_render_colors are [1,H,W,channels]; backgrounds [1,channels] as
+// rasterizer.cpp:272-298 builds them (zeros [1,1] for D / ED, cat(bg, 0) for RGB_D / RGB_ED).  The depth is not
+// differentiable (Ops.h:67): its colour-gradient column is dropped, and D / ED give sh0 / shN gradients of zero; a depth
+// loss still reaches means, rotation, scaling and opacity through the blend weights.  ED's division by alpha and the
+// image / depth split stay with the caller (rasterizer.cpp:367-420).  render_mode = RGB is the overload above.
+FusedForwardResult rasterize_from_world_fused_fwd(
+    const at::Tensor means, const at::Tensor sh0, const at::Tensor shN, const at::Tensor scaling_raw,
+    const at::Tensor rotation_raw, const at::Tensor opacity_raw, const uint32_t sh_degree, const float scaling_modifier,
+    const at::Tensor viewmat, const at::Tensor K, const uint32_t image_width, const uint32_t image_height,
+    const float eps2d, const float near_plane, const float far_plane, const float radius_clip,
+    const at::optional<at::Tensor> backgrounds, const CameraModelType camera_model,
+    const UnscentedTransformParameters ut_params, const at::optional<at::Tensor> radial_coeffs,
+    const at::optional<at::Tensor> tangential_coeffs, const at::optional<at::Tensor> thin_prism_coeffs,
+    const int64_t isect_capacity, const bool prepare_backward, const RenderMode render_mode);
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor> rasterize_from_world_fused_bwd(
+    const at::Tensor means, const at::Tensor sh0, const at::Tensor shN, const at::Tensor scaling_raw,
+    const at::Tensor rotation_raw, const at::Tensor opacity_raw, const uint32_t sh_degree, const float scaling_modifier,
+    const at::Tensor viewmat, const at::Tensor K, const uint32_t image_width, const uint32_t image_height,
+    const at::optional<at::Tensor> backgrounds, const CameraModelType camera_model,
+    const UnscentedTransformParameters ut_params, const at::optional<at::Tensor> radial_coeffs,
+    const at::optional<at::Tensor> tangential_coeffs, const at::optional<at::Tensor> thin_prism_coeffs,
+    const at::Tensor radii, const at::Tensor tile_offsets, const at::Tensor flatten_ids, at::Tensor workspace,
+    const at::Tensor render_alphas, const at::Tensor last_ids, const at::Tensor v_render_colors,
+    const at::Tensor v_render_alphas,
+    const at::Tensor depths, // the forward's FusedForwardResult::depths; read by RGB_D / RGB_ED only
+    const RenderMode render_mode);
 
 // SURVEY.md 8 (f2): loss = (1 - lambda) * l1(clamp(render, 0, 1), target) + lambda * (1 - fused_ssim(.., "valid")) of
 // src/training/trainer.cpp:103-126 and, when `compute_grad`, dLoss/d(renders) in the same kernel.
