@@ -48,10 +48,11 @@ CUDA_SOURCES = [
     ("gsb_adc.cu", []),
     ("gsb_sparsity.cu", []),
     ("gsb_metrics.cu", []),
+    ("gsb_knn.cu", ["-fmad=false"]),
 ]
 CUDA_HEADERS = ["gsb_common.cuh", "gsb_raster.cuh", "gsb_camera.cuh", "gsb_devsort.cuh", "gsb_sh.cuh", "gsb_projection.cuh", "gsb_ewa.cuh",
                 "gsb_relocation.cuh", "gsb_select.cuh", "gsb_scan.cuh", "gsb_reduce.cuh"]
-SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "Adc.cpp", "Sparsity.cpp", "Metrics.cpp", "torch_binding.cpp",
+SHIM_SOURCES = ["Ops.cpp", "FusedOps.cpp", "FastGs.cpp", "BilateralGrid.cpp", "Mcmc.cpp", "Adc.cpp", "Sparsity.cpp", "Metrics.cpp", "Init.cpp", "torch_binding.cpp",
                 "fastgs_binding.cpp"]
 
 

@@ -1,4 +1,5 @@
-// gsb_devsort.cuh -- device-wide radix sort of the intersect stage, hand-written for sm_90a.
+// gsb_devsort.cuh -- device-wide radix sort of the intersect stage and the neighbour search's cell order (gsb_knn.cu),
+// hand-written for sm_90a.
 //
 // Replaces the library sort of the reference's intersect_tile (cub::DeviceRadixSort::SortPairs,
 // gsplat/IntersectTile.cu:300-314) with this repository's own kernels:
@@ -177,6 +178,28 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(
         }
         __syncwarp();
     }
+}
+
+// Sorts n (key, value) pairs by key bits [begin_bit, end_bit), 8 per pass.  Without a control block the host alternates
+// the buffers: after an odd number of passes the result is in k1 / v1, after an even number in k0 / v0.
+template <typename KeyT>
+static inline int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, const ScanPlan &sp,
+                                    int passes, uint32_t begin_bit, uint32_t end_bit, const SortCtl *ctl, uint32_t *H,
+                                    cudaStream_t s) {
+    for (int pass = 0; pass < passes; ++pass) {
+        const uint32_t shift = begin_bit + 8u * (uint32_t)pass;
+        const uint32_t bits = end_bit - shift < 8u ? end_bit - shift : 8u;
+        const uint32_t mask = (1u << bits) - 1u;
+        // without a control block the host alternates the buffers itself
+        KeyT *ks = (!ctl && (pass & 1)) ? k1 : k0, *kd = (!ctl && (pass & 1)) ? k0 : k1;
+        uint32_t *vs = (!ctl && (pass & 1)) ? v1 : v0, *vd = (!ctl && (pass & 1)) ? v0 : v1;
+        radix_count_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, n, sp.seg, pass, shift, mask, ctl, H);
+        GSB_LAUNCH_CHECK();
+        radix_scatter_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, vs, vd, n, sp.seg, sp.nblocks, pass, shift,
+                                                                     mask, ctl, H);
+        GSB_LAUNCH_CHECK();
+    }
+    return GSB_OK;
 }
 
 } // namespace gsb

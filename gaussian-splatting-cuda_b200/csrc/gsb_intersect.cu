@@ -712,25 +712,6 @@ static PlanWs plan_ws(uint64_t n, const BinPlan &b, const ScanPlan &sp, bool fil
     return w;
 }
 
-template <typename KeyT>
-static int radix_sort_launch(KeyT *k0, KeyT *k1, uint32_t *v0, uint32_t *v1, uint64_t n, const ScanPlan &sp, int passes,
-                             uint32_t begin_bit, uint32_t end_bit, const SortCtl *ctl, uint32_t *H, cudaStream_t s) {
-    for (int pass = 0; pass < passes; ++pass) {
-        const uint32_t shift = begin_bit + 8u * (uint32_t)pass;
-        const uint32_t bits = end_bit - shift < 8u ? end_bit - shift : 8u;
-        const uint32_t mask = (1u << bits) - 1u;
-        // without a control block the host alternates the buffers itself
-        KeyT *ks = (!ctl && (pass & 1)) ? k1 : k0, *kd = (!ctl && (pass & 1)) ? k0 : k1;
-        uint32_t *vs = (!ctl && (pass & 1)) ? v1 : v0, *vd = (!ctl && (pass & 1)) ? v0 : v1;
-        radix_count_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, n, sp.seg, pass, shift, mask, ctl, H);
-        GSB_LAUNCH_CHECK();
-        radix_scatter_kernel<KeyT><<<sp.nblocks, kSortThreads, 0, s>>>(ks, kd, vs, vd, n, sp.seg, sp.nblocks, pass, shift,
-                                                                     mask, ctl, H);
-        GSB_LAUNCH_CHECK();
-    }
-    return GSB_OK;
-}
-
 } // namespace gsb
 
 extern "C" size_t gsb_isect_count_workspace(uint64_t n_elements) {

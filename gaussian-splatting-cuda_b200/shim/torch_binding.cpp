@@ -256,6 +256,12 @@ void image_metrics(const Tensor &image, const Tensor &target, bool image_hwc, Te
     gsplat::image_metrics(image, target, image_hwc, out);
 }
 
+Tensor mean_neighbor_distances(const Tensor &points) { return gsplat::mean_neighbor_distances(points); }
+
+void mean_neighbor_distances_out(const Tensor &points, Tensor out, Tensor status) {
+    gsplat::mean_neighbor_distances_out(points, out, status);
+}
+
 } // namespace
 
 TORCH_LIBRARY(gsplat_b200, m) {
@@ -300,4 +306,7 @@ TORCH_LIBRARY(gsplat_b200, m) {
     m.def("add_noise(Tensor raw_opacities, Tensor raw_scales, Tensor raw_quats, Tensor noise, Tensor(a!) means, float current_lr) -> ()",
           &add_noise);
     m.def("image_metrics(Tensor image, Tensor target, bool image_hwc, Tensor(a!) out) -> ()", &image_metrics);
+    m.def("mean_neighbor_distances", &mean_neighbor_distances);
+    m.def("mean_neighbor_distances_out(Tensor points, Tensor(a!) out, Tensor(b!) status) -> ()",
+          &mean_neighbor_distances_out);
 }

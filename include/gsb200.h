@@ -632,6 +632,23 @@ GSB_API size_t gsb_image_metrics_workspace(void);
 GSB_API int gsb_image_metrics(uint32_t W, uint32_t H, const float *image, const float *target, uint32_t flags,
                               float *out /*DEVICE [2]*/, void *workspace, size_t workspace_bytes, gsb_stream_t stream);
 
+/* ---- Model set-up: initial scales (src/core/splat_data.cpp:63-111, compute_mean_neighbor_distances) ------------------
+ * gsb_knn_mean_dist: for each of the N points (DEVICE float[N,3]) the mean distance to its nearest neighbours, into out
+ * (DEVICE float[N]), computed exactly (the reference's nanoflann query uses eps = 10 and is approximate):
+ *   the k = min(4, N) smallest squared distances over all points, the point itself and its duplicates included, each
+ *   ((dx*dx) + (dy*dy)) + (dz*dz) in float32 without FMA, dx = q.x - p.x; walked in ascending order, the first (at most
+ *   3) with d2 > 1e-8f are averaged as sqrtf values summed in float32 in that order; 0.01f when none qualifies.
+ * status (DEVICE uint32[1]) is written on the stream: 0, or GSB_KNN_NONFINITE when a coordinate is NaN or infinite (out
+ * is then unspecified).  N == 0 only writes status.  N at most GSB_KNN_MAX_POINTS.  Workspace:
+ * gsb_knn_mean_dist_workspace(N) bytes, 256-aligned; its counters are reset on the stream, so the call can be captured
+ * in a CUDA graph.  Each value depends only on the point set, not on the search order: repeated calls give the same
+ * bits. */
+enum { GSB_KNN_NONFINITE = 1 };
+#define GSB_KNN_MAX_POINTS (1u << 28)
+GSB_API size_t gsb_knn_mean_dist_workspace(uint32_t N);
+GSB_API int gsb_knn_mean_dist(uint32_t N, const float *points, float *out, void *workspace, size_t workspace_bytes,
+                              uint32_t *status /*DEVICE [1]*/, gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -199,4 +199,14 @@ std::tuple<at::Tensor, at::Tensor> sparsity_prune_classify(const at::Tensor opac
 // image: [3,H,W], or [H,W,3] (the from-world blend's layout, read in place) when image_hwc.
 void image_metrics(const at::Tensor image, const at::Tensor target, const bool image_hwc, at::Tensor out);
 
+// Model set-up (src/core/splat_data.cpp:63-111, compute_mean_neighbor_distances): for each point of points [N,3]
+// (float32, CUDA) the mean distance to its nearest neighbours, [N] float32 on the device.  The same semantics as the
+// reference's function, but the search is exact where the reference's (nanoflann, eps = 10) is approximate: the first
+// (up to 3) of the min(4, N) smallest squared distances, the point itself included, that exceed 1e-8; 0.01 when none
+// does.  Raises c10::Error on a bad shape, dtype or device, or on a NaN or infinite coordinate (one read-back).
+at::Tensor mean_neighbor_distances(const at::Tensor points);
+// The same into out [N] float32, with status [1] int32 set to 0 or GSB_KNN_NONFINITE on the device and not read back,
+// so the call can be captured in a CUDA graph.
+void mean_neighbor_distances_out(const at::Tensor points, at::Tensor out, at::Tensor status);
+
 } // namespace gsplat
