@@ -13,6 +13,9 @@
 // no 2-million-element reductions go through HBM.  Every stage is cut into about 256 strips (one per thread) and is
 // input-stationary -- an input is read from shared memory once and added to every output whose window covers it -- so
 // a thread keeps a handful of accumulators instead of a row of inputs (64 registers, three CTAs per SM).
+// A NaN render propagates as in the reference: the clamp keeps it, so the loss is NaN and so is the gradient of its
+// channel within 10 pixels of it; the clamp mask (0 <= raw <= 1, false for NaN) gives the NaN pixel itself a zero gradient, as torch's
+// clamp backward does.
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -63,6 +66,15 @@ struct LossSmem {
 static_assert(sizeof(float2) * kSH * kTP <= sizeof(float2) * (kIH + 1) * kSP, "g01 alias");
 static_assert(sizeof(float) * kSH * kTP <= sizeof(float) * (kIH + 1) * kSP, "g2 alias");
 
+// clamp(v, 0, 1) as torch::clamp computes it: NaN stays NaN.  fminf / fmaxf would make NaN 0 (nvcc folds them into one
+// saturating add, which does the same); the NaN-propagating min / max cost one instruction more, and the clamp mask
+// below then needs one comparison instead of two.
+__device__ __forceinline__ float clamp01_keep_nan(float v) {
+    asm("max.NaN.f32 %0, %0, 0f00000000;" : "+f"(v));
+    asm("min.NaN.f32 %0, %0, 0f3F800000;" : "+f"(v));
+    return v;
+}
+
 // NoClamp (GSB_LOSS_NO_CLAMP): the renders enter as they are and every pixel passes the gradient
 template <bool NoClamp>
 __global__ void __launch_bounds__(kLossThreads, 3) ssim_l1_kernel(const LossParams p) {
@@ -102,11 +114,12 @@ __global__ void __launch_bounds__(kLossThreads, 3) ssim_l1_kernel(const LossPara
                     float X = 0.f, Y = 0.f;
                     if (row_ok && gx >= 0 && gx < W) {
                         const float raw = rrow[gx * rstep];
-                        X = NoClamp ? raw : fminf(fmaxf(raw, 0.f), 1.f);
+                        X = NoClamp ? raw : clamp01_keep_nan(raw);
                         Y = trow[gx * tstep];
-                        // the tile's own pixels remember whether the clamp was active (dLoss/d(render) = 0 there)
+                        // the tile's own pixels remember whether the clamp was active (dLoss/d(render) = 0 there):
+                        // X == raw is 0 <= raw <= 1 (-0 included, NaN not), torch's clamp-backward mask
                         const int tr = r - 2 * kHalo, tq = q - 2 * kHalo;
-                        if (tr >= 0 && tr < kTH && tq >= 0 && tq < kTW) s_pass[tr][tq] = (NoClamp || (raw >= 0.f && raw <= 1.f)) ? 1 : 0;
+                        if (tr >= 0 && tr < kTH && tq >= 0 && tq < kTW) s_pass[tr][tq] = (NoClamp || X == raw) ? 1 : 0;
                     }
                     S.xy[r][q] = make_float2(X, Y);
                 }

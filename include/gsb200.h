@@ -378,7 +378,9 @@ GSB_API int gsb_fused_back_mode(const GsbSplatRaw *splats, const GsbCamera *cam,
  * v_renders (laid out like renders) = grad_scale * dLoss/d(renders) including the clamp mask, or NULL to evaluate only.
  * loss_out: DEVICE float[3] = (loss, l1 mean, ssim mean).  workspace: gsb_ssim_l1_workspace() bytes, 256-aligned.
  * GSB_LOSS_NO_CLAMP (4): the renders are used as they are -- no clamp and no clamp mask -- as the reference's loss
- * treats an image that went through the bilateral grid (trainer.cpp:662-665 -> 103-126). */
+ * treats an image that went through the bilateral grid (trainer.cpp:662-665 -> 103-126).
+ * NaN propagates: a NaN render makes the loss NaN (the clamp keeps NaN, as torch::clamp does).  Its own gradient is 0
+ * with the clamp (the mask 0 <= render <= 1 is false there) and NaN with GSB_LOSS_NO_CLAMP. */
 enum { GSB_LOSS_TARGET_CHW = 1, GSB_LOSS_RENDERS_CHW = 2, GSB_LOSS_NO_CLAMP = 4 };
 GSB_API size_t gsb_ssim_l1_workspace(void);
 GSB_API int gsb_ssim_l1(uint32_t image_width, uint32_t image_height, const float *renders, const float *target,

@@ -7,30 +7,11 @@ import numpy as np
 import pytest
 import torch
 
+import loss_restatement as lr
 import scenes
 from parity import rel, to_dev
 
 pytestmark = pytest.mark.gpu
-
-
-def torch_loss(renders, target_chw, lam):
-    """float64 restatement: clamp, permute, L1 mean, 11x11 Gaussian SSIM with zero padding, 'valid' crop, mean."""
-    img = torch.clamp(renders[0].permute(2, 0, 1), 0.0, 1.0).double()[None]  # [1,3,H,W]
-    gt = target_chw.double()[None]
-    x = torch.arange(11, dtype=torch.float64, device=renders.device) - 5
-    g = torch.exp(-(x ** 2) / (2 * 1.5 ** 2))
-    g = (g / g.sum())
-    win = (g[:, None] * g[None, :])[None, None].repeat(3, 1, 1, 1)
-    conv = lambda t: torch.nn.functional.conv2d(t, win, padding=5, groups=3)
-    mu1, mu2 = conv(img), conv(gt)
-    s1, s2, s12 = conv(img * img) - mu1 * mu1, conv(gt * gt) - mu2 * mu2, conv(img * gt) - mu1 * mu2
-    C1, C2 = 0.01 ** 2, 0.03 ** 2
-    m = ((2 * mu1 * mu2 + C1) * (2 * s12 + C2)) / ((mu1 * mu1 + mu2 * mu2 + C1) * (s1 + s2 + C2))
-    H, W = m.shape[-2:]
-    if H > 10 and W > 10:
-        m = m[..., 5:H - 5, 5:W - 5]
-    l1 = (img - gt).abs().mean()
-    return (1 - lam) * l1 + lam * (1 - m.mean()), l1, m.mean()
 
 
 @pytest.mark.parametrize("H,W", [(64, 80), (70, 150), (9, 40), (270, 480)])
@@ -41,14 +22,13 @@ def test_photometric_loss_and_gradient_vs_torch(native, cuda_device, H, W):
     target = torch.rand((3, H, W), device=cuda_device, generator=g)
     loss, stats = training.photometric_loss(renders, target, 0.2)
     (loss * 1.7).backward()
-    r64 = renders.detach().clone().requires_grad_(True)
-    want, l1, ssim = torch_loss(r64, target, 0.2)
-    (want * 1.7).backward()
-    print(f"[{H}x{W}] loss {float(loss):.6f} vs torch f64 {float(want):.6f}; grad rel_l2 {rel(renders.grad, r64.grad):.2e}")
-    assert abs(float(loss) - float(want)) < 2e-6 * max(1.0, abs(float(want)))
-    assert abs(float(stats[1]) - float(l1)) < 2e-6 and abs(float(stats[2]) - float(ssim)) < 2e-6
-    assert rel(renders.grad, r64.grad) < 2e-5
-    assert float((renders.grad - r64.grad.float()).abs().max()) < 1e-4 * float(r64.grad.abs().max())
+    want, l1, ssim, g64 = lr.photometric_loss_f64(renders, target, 0.2)
+    g64 = 1.7 * g64
+    print(f"[{H}x{W}] loss {float(loss):.6f} vs torch f64 {want:.6f}; grad rel_l2 {rel(renders.grad, g64):.2e}")
+    assert abs(float(loss) - want) < 2e-6 * max(1.0, abs(want))
+    assert abs(float(stats[1]) - l1) < 2e-6 and abs(float(stats[2]) - ssim) < 2e-6
+    assert rel(renders.grad, g64) < 2e-5
+    assert float((renders.grad - g64.float()).abs().max()) < 1e-4 * float(g64.abs().max())
     # the same target in the blend's own layout
     loss2, _ = training.photometric_loss(renders.detach(), target.permute(1, 2, 0)[None].contiguous(), 0.2)
     assert abs(float(loss2) - float(loss)) < 1e-7
@@ -165,7 +145,7 @@ def ref_train(native):
     return rt
 
 
-@pytest.mark.parametrize("H,W", [(70, 150), (540, 960)])
+@pytest.mark.parametrize("H,W", [(11, 11), (17, 33), (70, 150), (540, 960), (1080, 1920)])
 def test_photometric_loss_vs_reference_kernels(native, ref_train, cuda_device, H, W):
     from gsplat_b200 import training
     g = torch.Generator(device=cuda_device).manual_seed(7)
