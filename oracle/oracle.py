@@ -294,11 +294,14 @@ def add_noise(raw_opacities, raw_scales, raw_quats, noise, means, current_lr, pr
 # ---------------------------------------------------------------------------------------------
 
 def render_pipeline(scene: dict, precision="f32", with_bwd=False, v_render_colors=None,
-                    v_render_alphas=None, viewmats1=None, rs_type=GLOBAL):
+                    v_render_alphas=None, viewmats1=None, rs_type=GLOBAL, camera_model=PINHOLE, radial=None,
+                    tangential=None, thin_prism=None):
     """Run projection -> SH -> intersect -> blend (and optionally the backward chain through
     blend bwd and SH bwd) on a scene dict made by tests/scenes.py. C == 1.  viewmats1 / rs_type: a rolling
-    shutter's end-of-frame pose and direction (the SH directions use the start pose's camera centre)."""
-    rs = dict(viewmats1=viewmats1, rs_type=rs_type)
+    shutter's end-of-frame pose and direction (the SH directions use the start pose's camera centre).
+    camera_model and the distortion coefficients as projection_ut takes them."""
+    rs = dict(viewmats1=viewmats1, rs_type=rs_type, camera_model=camera_model, radial=radial, tangential=tangential,
+              thin_prism=thin_prism)
     W, H, ts = scene["width"], scene["height"], scene.get("tile_size", 16)
     tw, th = (W + ts - 1) // ts, (H + ts - 1) // ts
     means, quats, scales, opac = scene["means"], scene["quats"], scene["scales"], scene["opacities"]
@@ -329,7 +332,7 @@ def render_pipeline(scene: dict, precision="f32", with_bwd=False, v_render_color
 
 
 def backward_pipeline(scene: dict, out: dict, v_render_colors, v_render_alphas, precision="f32", viewmats1=None,
-                      rs_type=GLOBAL):
+                      rs_type=GLOBAL, camera_model=PINHOLE, radial=None, tangential=None, thin_prism=None):
     """Backward chain of render_pipeline's forward `out` (blend bwd -> clamp -> SH bwd); adds the
     gradients to `out` in place and returns it."""
     W, H, ts = scene["width"], scene["height"], scene.get("tile_size", 16)
@@ -338,10 +341,12 @@ def backward_pipeline(scene: dict, out: dict, v_render_colors, v_render_alphas, 
     g = raster_bwd(means, quats, scales, out["colors"], opac[None], scene.get("background"), None, W, H, ts,
                    scene["viewmats"], scene["Ks"], out["tile_offsets"], out["flatten_ids"], out["alphas"],
                    out["last_ids"], v_render_colors, v_render_alphas, precision=precision, viewmats1=viewmats1,
-                   rs_type=rs_type)
+                   rs_type=rs_type, camera_model=camera_model, radial=radial, tangential=tangential,
+                   thin_prism=thin_prism)
     out.update(v_means=g[0], v_quats=g[1], v_scales=g[2], v_colors=g[3], v_opacities=g[4])
-    # clamp_min(+0.5) backward, then SH backward (rasterizer_autograd.cpp:84-132)
-    v_sh_colors = (g[3] * ((out["sh_colors"] + 0.5) > 0)).astype(np.float32)
+    # clamp_min(+0.5) backward, then SH backward (rasterizer_autograd.cpp:84-132).  torch's clamp_min passes the
+    # gradient where its argument is >= the bound, so a colour of exactly -0.5 still gets it
+    v_sh_colors = (g[3] * ((out["sh_colors"] + 0.5) >= 0)).astype(np.float32)
     v_coeffs, v_dirs = sh_bwd(deg, out["dirs"], np.broadcast_to(sh[None], (1,) + sh.shape), out["masks"],
                               v_sh_colors, True, precision=precision)
     out.update(v_sh_coeffs=v_coeffs[0], v_dirs=v_dirs)
